@@ -142,6 +142,63 @@ struct GroupOps<32> {
     return v;
   }
 };
+// ---- transposed moment reductions ------------------------------------------------------------------
+// Sum of N doubles per lane over an aligned group of D*2 lanes as a reduce-scatter: at the step of distance d a lane keeps
+// one half of its values (the lower half if lane bit d is clear, else the upper half) and receives the partner's partial
+// of that half, so the values exchanged halve with every step (N = 9: 12 shuffles, 18: 20) instead of N per step. Once
+// one value is left the remaining steps are plain butterflies. Every partial is the sum the xor butterfly forms at the
+// same step (lane + lane ^ d, and IEEE addition commutes), so each total is bit-identical to warp_sum / GroupOps::sum_d,
+// in every lane that holds it. Afterwards quantity q is in slot rs_slot(N, D, q) of lane rs_lane(N, D, q) of the group.
+// (not recursive, so that the compiler folds them at the unrolled call sites)
+__host__ __device__ __forceinline__ constexpr int rs_lane(int n, int d, int q) {
+  int l = 0;
+  for (; d > 0 && n > 1; d >>= 1) { const int h = (n + 1) / 2; if (q >= h) { l |= d; q -= h; } n = h; }
+  return l;
+}
+__host__ __device__ __forceinline__ constexpr int rs_slot(int n, int d, int q) {
+  for (; d > 0 && n > 1; d >>= 1) { const int h = (n + 1) / 2; if (q >= h) q -= h; n = h; }
+  return q;
+}
+template <int N, int D, int CAP>
+__device__ __forceinline__ void reduce_scatter(double (&v)[CAP], int lane) {
+  if constexpr (D > 0) {
+    if constexpr (N == 1) {
+      v[0] += __shfl_xor_sync(0xffffffffu, v[0], D);
+      reduce_scatter<1, D / 2>(v, lane);
+    } else {
+      constexpr int H = (N + 1) / 2;
+      const bool up = (lane & D) != 0;
+#pragma unroll
+      for (int k = 0; k < H; ++k) {
+        const double lo = v[k], hi = (k + H < N) ? v[(k + H < N) ? k + H : 0] : 0.0;
+        const double r = __shfl_xor_sync(0xffffffffu, up ? lo : hi, D);
+        v[k] = (up ? hi : lo) + r;
+      }
+      reduce_scatter<H, D / 2>(v, lane);
+    }
+  }
+}
+// Group-wide sums of v[0..N) in every lane of the group of G lanes: reduce-scatter, then one shuffle per quantity.
+template <int N, int G>
+__device__ __forceinline__ void group_sum_all(double (&v)[N], int lane) {
+  reduce_scatter<N, G / 2>(v, lane);
+  double r[N];
+#pragma unroll
+  for (int q = 0; q < N; ++q) r[q] = __shfl_sync(0xffffffffu, v[rs_slot(N, G / 2, q)], rs_lane(N, G / 2, q), G);
+#pragma unroll
+  for (int q = 0; q < N; ++q) v[q] = r[q];
+}
+// the 9 moment sums of m over the group (m.n is left alone)
+template <int G>
+__device__ __forceinline__ void group_sum_moments(Moments& m, int lane) {
+  double v[9] = {m.s1[0], m.s1[1], m.s1[2], m.s2[0], m.s2[1], m.s2[2], m.s2[3], m.s2[4], m.s2[5]};
+  group_sum_all<9, G>(v, lane);
+#pragma unroll
+  for (int q = 0; q < 3; ++q) m.s1[q] = v[q];
+#pragma unroll
+  for (int q = 0; q < 6; ++q) m.s2[q] = v[3 + q];
+}
+
 enum FitState { ST_RVPF = 0, ST_SEED = 1, ST_GPF = 2, ST_FINAL = 3, ST_DONE = 4 };
 
 // The register-resident fit kernel (classes S and M). G lanes cooperate on one patch, K points per lane; a warp
@@ -198,7 +255,8 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
     unsigned amask = vmask;                    // alive = not removed by R-VPF (S:495-504)
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
-    const double margin_z = have ? ap.adaptive_seed_selection_margin * states[f].sensor_height : 0.0;  // S:90
+    // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
+    const float margin_f = (have && zone0) ? float_ru(ap.adaptive_seed_selection_margin * states[f].sensor_height) : -INFINITY;
     double c0x = 0.0, c0y = 0.0;               // first point: reference point of the shifted moments of the seed fits
     if (have) { const float4 p = P[0]; c0x = (double) p.x; c0y = (double) p.y; }
 
@@ -218,7 +276,7 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
       const bool seed_round = active && (state == ST_RVPF || state == ST_SEED);
       const bool seed_round_was_rvpf = (state == ST_RVPF);
       double c[3] = {pl.mean[0], pl.mean[1], pl.mean[2]};
-      double zthr = 0.0;
+      float zthr = 0.f;   // float_ru of the seed threshold
       // (1) LPR selection for seed rounds: 32-step bisection on order-preserving keys with group-wide counting
       if (__any_sync(0xffffffffu, seed_round)) {
         unsigned smask = 0;  // candidates: alive and not below the zone-0 margin (S:88-96)
@@ -226,7 +284,7 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
 #pragma unroll
         for (int k = 0; k < K; ++k) {
           keys[k] = order_key(pz[k]);
-          const bool ok = seed_round && ((amask >> k) & 1u) && !(zone0 && ((double) pz[k] < margin_z));
+          const bool ok = seed_round && ((amask >> k) & 1u) && !(pz[k] < margin_f);
           smask |= ok ? (1u << k) : 0u;
         }
         const int nvalid = Ops::sum_i(__popc(smask), nullptr);
@@ -262,7 +320,7 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
         double lpr = 0.0;
         if (target > 0) lpr = (part_sum + (double) (target - c_lt) * (double) key_to_float(ans)) / (double) target;
         if (seed_round) {
-          zthr = lpr + (state == ST_RVPF ? ap.th_seeds_v : ap.th_seeds);
+          zthr = float_ru(lpr + (state == ST_RVPF ? ap.th_seeds_v : ap.th_seeds));
           c[0] = c0x; c[1] = c0y; c[2] = lpr;
         }
       }
@@ -279,7 +337,7 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
         for (int k = 0; k < K; ++k) {
           if (k >= kmax) break;
           bool in = (amask >> k) & 1u;
-          if (seed_round) in = in && ((double) pz[k] < zthr);                                          // S:108 / S:145
+          if (seed_round) in = in && (pz[k] < zthr);                                                   // S:108 / S:145
           else in = in && have_plane && (point_plane_distance(pl, px[k], py[k], pz[k]) < ap.th_dist);  // S:525 / S:529
           if (in) {
             sel |= 1u << k;
@@ -291,10 +349,7 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
           }
         }
       }
-#pragma unroll
-      for (int q = 0; q < 3; ++q) m.s1[q] = Ops::sum_d(m.s1[q], nullptr);
-#pragma unroll
-      for (int q = 0; q < 6; ++q) m.s2[q] = Ops::sum_d(m.s2[q], nullptr);
+      group_sum_moments<G>(m, lane);
       m.n = Ops::sum_i(m.n, nullptr);
       // every lane of the warp takes part in this reduction (the groups of a warp are in different states)
       const bool set_unchanged = Ops::sum_i((active && sel != prev_sel) ? 1 : 0, nullptr) == 0;
@@ -453,7 +508,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
     unsigned amask = vmask;
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
-    const double margin_z = ap.adaptive_seed_selection_margin * states[f].sensor_height;  // S:90
+    // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
+    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[f].sensor_height) : -INFINITY;
     const float4 first = P[0];
     const double c0x = (double) first.x, c0y = (double) first.y;
 
@@ -485,7 +541,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
       const bool seed_round = (state == ST_RVPF || state == ST_SEED);
       const bool fused = fuse_ok && state == ST_RVPF;
       double c[3] = {pl.mean[0], pl.mean[1], pl.mean[2]};
-      double zthr = 0.0, zin = 0.0;
+      float zthr = 0.f, zin = 0.f;   // float_ru of the seed thresholds
       if (seed_round) {
         // ---- LPR: mean of the num_lpr lowest z among the alive points not below the zone-0 margin (S:88-103) ----
         unsigned smask = 0, kmin = 0xffffffffu;
@@ -493,7 +549,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         for (int it = 0; it < nit; ++it) {
           if (!((amask >> it) & 1u)) continue;
           const float z = sz[jbase + it * 32];
-          if (zone0 && ((double) z < margin_z)) continue;
+          if (z < margin_f) continue;
           smask |= 1u << it;
           const unsigned key = order_key(z);
           kmin = key < kmin ? key : kmin;
@@ -604,8 +660,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
           __syncthreads();
         }
         const double lpr = s_lpr;
-        zthr = lpr + (state == ST_RVPF ? ap.th_seeds_v : ap.th_seeds);
-        zin = lpr + ap.th_seeds;
+        zthr = float_ru(lpr + (state == ST_RVPF ? ap.th_seeds_v : ap.th_seeds));
+        zin = float_ru(lpr + ap.th_seeds);
         c[0] = c0x; c[1] = c0y; c[2] = lpr;
       }
       // ---- predicate + moments ----
@@ -630,7 +686,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         const int j = jbase + it * 32;
         const float x = sx[j], y = sy[j], z = sz[j];
         bool in;
-        if (seed_round) in = ((double) z < zthr);                                            // S:108 / S:145
+        if (seed_round) in = (z < zthr);                                                     // S:108 / S:145
         else {
           int fl = have_plane ? dist_filter(pf, thf, x, y, z) : 0;
           if (fl < 0) fl = (point_plane_distance(pl, x, y, z) < ap.th_dist) ? 1 : 0;         // S:525 / S:529, exact
@@ -649,7 +705,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         a[0] += wx; a[1] += wy; a[2] += wz;
         a[3] += wx * dx; a[4] += wx * dy; a[5] += wx * dz; a[6] += wy * dy; a[7] += wy * dz; a[8] += wz * dz;
         mn += in ? 1 : -1;
-        if (FUSE && fused && ((double) z < zin)) {   // also a seed of the R-GPF seed fit (in is true here)
+        if (FUSE && fused && (z < zin)) {   // also a seed of the R-GPF seed fit (in is true here)
           seli |= 1u << it;
           bi[0] += dx; bi[1] += dy; bi[2] += dz;
           bi[3] += dx * dx; bi[4] += dx * dy; bi[5] += dx * dz; bi[6] += dy * dy; bi[7] += dy * dz; bi[8] += dz * dz;
@@ -657,31 +713,30 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         }
       }
       member = (FUSE && fused) ? seli : sel;   // a fused round that is not taken recomputes everything in the next round
-#pragma unroll
-      for (int q = 0; q < 9; ++q) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) a[q] += __shfl_xor_sync(0xffffffffu, a[q], o);
-      }
       mn = __reduce_add_sync(0xffffffffu, mn);
       nchg = __reduce_add_sync(0xffffffffu, nchg);
       const int buf = round & 1;
       ++round;
+      // warp sums by reduce-scatter: the lane that ends up holding quantity q stores it
       if (FUSE && fused) {
+        double v[18];
 #pragma unroll
-        for (int q = 0; q < (FUSE ? 9 : 1); ++q) {
+        for (int q = 0; q < 9; ++q) { v[q] = a[q]; v[9 + q] = bi[FUSE ? q : 0]; }
+        reduce_scatter<18, 16>(v, lane);
 #pragma unroll
-          for (int o = 16; o > 0; o >>= 1) bi[q] += __shfl_xor_sync(0xffffffffu, bi[q], o);
+        for (int q = 0; q < 9; ++q) {
+          if (lane == rs_lane(18, 16, q)) s_part[buf][w][q] = v[rs_slot(18, 16, q)];
+          if (lane == rs_lane(18, 16, 9 + q)) s_parti[FUSE ? buf : 0][FUSE ? w : 0][q] = v[rs_slot(18, 16, 9 + q)];
         }
         mni = __reduce_add_sync(0xffffffffu, mni);
-        if (lane == 0) {
+        if (lane == 0) s_cnt[w][1] = mni;
+      } else {
+        reduce_scatter<9, 16>(a, lane);
 #pragma unroll
-          for (int q = 0; q < (FUSE ? 9 : 1); ++q) s_parti[FUSE ? buf : 0][FUSE ? w : 0][q] = bi[q];
-          s_cnt[w][1] = mni;
-        }
+        for (int q = 0; q < 9; ++q)
+          if (lane == rs_lane(9, 16, q)) s_part[buf][w][q] = a[rs_slot(9, 16, q)];
       }
       if (lane == 0) {
-#pragma unroll
-        for (int q = 0; q < 9; ++q) s_part[buf][w][q] = a[q];
         s_pcnt[buf][w] = mn;
         s_pchg[buf][w] = nchg;
       }
@@ -942,8 +997,8 @@ constexpr int FITW_U = 4;                       // loads in flight per lane
 
 // Rare path of warp_lpr (num_lpr > 32, or more than 128 points tie below the bound): streaming selector with a
 // bitonic sort of the candidate buffer. Kept out of line so that its ~2000 instructions stay out of the hot code.
-__device__ __noinline__ double warp_lpr_fallback(const float4* __restrict__ P, int n, int nit, bool any_removed, const unsigned* __restrict__ alive_w, bool zone0,
-                                                 double margin_z, int num_lpr, float* sel_buf) {
+__device__ __noinline__ double warp_lpr_fallback(const float4* __restrict__ P, int n, int nit, bool any_removed, const unsigned* __restrict__ alive_w,
+                                                 float margin_f, int num_lpr, float* sel_buf) {
   const int lane = lane_id();
   double lpr = 0.0;
   LprSelector sel;
@@ -953,7 +1008,7 @@ __device__ __noinline__ double warp_lpr_fallback(const float4* __restrict__ P, i
     bool valid = j < n;
     const float z = P[j < n ? j : n - 1].z;
     if (any_removed) valid = valid && ((alive_w[it] >> lane) & 1u);
-    if (zone0 && ((double) z < margin_z)) valid = false;
+    if (z < margin_f) valid = false;
     sel.push(valid, z);
   }
   sel.prune();
@@ -967,12 +1022,12 @@ __device__ __noinline__ double warp_lpr_fallback(const float4* __restrict__ P, i
 }
 
 // LPR height for one warp-owned patch (extract_initial_seeds, S:84-103): mean of the (<= num_lpr) lowest z among
-// the points that are alive and, in zone 0, not below the adaptive margin.
+// the points that are alive and not below margin_f (float_ru of the zone-0 adaptive margin, -inf in the other zones).
 // Two-level selection: the num_lpr-th smallest of the 32 per-lane minima is an upper bound T of the num_lpr-th
 // smallest point, so only the few points with z <= T are gathered (ballot append into the warp's 128-slot buffer)
 // and the exact k-th key is bisected among them. Falls back to the streaming selector when num_lpr > 32 or when
 // more than 128 points tie below the bound.
-__device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool any_removed, const unsigned* __restrict__ alive_w, bool zone0, double margin_z,
+__device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool any_removed, const unsigned* __restrict__ alive_w, float margin_f,
                            int num_lpr, float* sel_buf) {
   const int lane = lane_id();
   const unsigned lt = lanemask_lt();
@@ -996,7 +1051,7 @@ __device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool an
         bool valid = j < n;
         const float z = zb[u];
         if (any_removed && it < nit) valid = valid && ((alive_w[it] >> lane) & 1u);
-        if (zone0 && ((double) z < margin_z)) valid = false;
+        if (z < margin_f) valid = false;
         if (valid) { kminL = min(kminL, order_key(z)); ++nv; }
       }
     }
@@ -1021,7 +1076,7 @@ __device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool an
         bool valid = j < n;
         const float z = zb[u];
         if (any_removed && it < nit) valid = valid && ((alive_w[it] >> lane) & 1u);
-        if (zone0 && ((double) z < margin_z)) valid = false;
+        if (z < margin_f) valid = false;
         const unsigned key = order_key(z);
         const bool c = valid && key <= T;
         const unsigned bal = __ballot_sync(0xffffffffu, c);
@@ -1057,7 +1112,7 @@ __device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool an
       __syncwarp();
     } else fallback = true;
   }
-  if (fallback) lpr = warp_lpr_fallback(P, n, nit, any_removed, alive_w, zone0, margin_z, num_lpr, sel_buf);
+  if (fallback) lpr = warp_lpr_fallback(P, n, nit, any_removed, alive_w, margin_f, num_lpr, sel_buf);
   return lpr;
 }
 
@@ -1129,7 +1184,8 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
     }
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
-    const double margin_z = ap.adaptive_seed_selection_margin * states[f].sensor_height;  // S:90
+    // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
+    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[f].sensor_height) : -INFINITY;
     const float4 first = P[0];
     double c[3] = {(double) first.x, (double) first.y, 0.0};   // reference point of all moment sums of this patch
 
@@ -1163,9 +1219,9 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
       const bool rvpf_round = rvpf_left > 0;
       const bool fused = fuse_ok && rvpf_round;
       // LPR: mean of the num_lpr lowest z among the alive points not below the zone-0 margin (S:88-103)
-      const double lpr = warp_lpr(P, n, nit, any_removed, alive_w, zone0, margin_z, ap.num_lpr, sel_buf);
-      const double zthr = lpr + (rvpf_round ? ap.th_seeds_v : ap.th_seeds);
-      const double zin = lpr + ap.th_seeds;   // inner (R-GPF seed) threshold of a fused round
+      const double lpr = warp_lpr(P, n, nit, any_removed, alive_w, margin_f, ap.num_lpr, sel_buf);
+      const float zthr = float_ru(lpr + (rvpf_round ? ap.th_seeds_v : ap.th_seeds));
+      const float zin = float_ru(lpr + ap.th_seeds);   // inner (R-GPF seed) threshold of a fused round
       c[2] = lpr;
       if (!looked_ahead) {   // the claim issued at the top has returned by now: fetch the next patch's descriptor
         const int t_next = __shfl_sync(0xffffffffu, next_raw, 0);
@@ -1187,12 +1243,12 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
         for (int u = 0; u < U; ++u) {
           const int j = (it + u) * 32 + lane;
           const float4 p = q[u];
-          bool in = (j < n) && ((double) p.z < zthr);                                     // S:108 / S:145
+          bool in = (j < n) && (p.z < zthr);                                              // S:108 / S:145
           if (any_removed && it + u < nit) in = in && ((alive_w[it + u] >> lane) & 1u);
           const unsigned bal = __ballot_sync(0xffffffffu, in);
           unsigned bal_in = bal;   // what becomes the member set: the inner set in a fused round
           bool inner = in;
-          if (FUSE && fused) { inner = in && ((double) p.z < zin); bal_in = __ballot_sync(0xffffffffu, inner); }
+          if (FUSE && fused) { inner = in && (p.z < zin); bal_in = __ballot_sync(0xffffffffu, inner); }
           if (lane == 0 && it + u < nit) member_w[it + u] = bal_in;
           if (bal) {
             const double w = in ? 1.0 : 0.0;   // unselected lanes add exact zeros
@@ -1212,16 +1268,10 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
           }
         }
       }
-#pragma unroll
-      for (int q = 0; q < 3; ++q) m.s1[q] = warp_sum(m.s1[q]);
-#pragma unroll
-      for (int q = 0; q < 6; ++q) m.s2[q] = warp_sum(m.s2[q]);
+      group_sum_moments<32>(m, lane);
       m.n = warp_sum_i(m.n);
       if (FUSE && fused) {
-#pragma unroll
-        for (int q = 0; q < 3; ++q) mi.s1[q] = warp_sum(mi.s1[q]);
-#pragma unroll
-        for (int q = 0; q < 6; ++q) mi.s2[q] = warp_sum(mi.s2[q]);
+        group_sum_moments<32>(mi, lane);
         mi.n = warp_sum_i(mi.n);
         // lanes 0..15 solve the R-VPF plane (all seeds), lanes 16..31 the R-GPF seed plane (inner seeds)
         const bool hi = lane >= 16;
@@ -1315,11 +1365,12 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
       }
       if (changed_any == 0) break;   // fixpoint: every later iteration would reproduce this set and this plane
       {
+        group_sum_moments<32>(dm, lane);
         Moments t = tot;
 #pragma unroll
-        for (int q = 0; q < 3; ++q) t.s1[q] += warp_sum(dm.s1[q]);
+        for (int q = 0; q < 3; ++q) t.s1[q] += dm.s1[q];
 #pragma unroll
-        for (int q = 0; q < 6; ++q) t.s2[q] += warp_sum(dm.s2[q]);
+        for (int q = 0; q < 6; ++q) t.s2[q] += dm.s2[q];
         t.n += warp_sum_i(dm.n);
         set_tot(t);
         if (t.n > 0) { Plane np; plane_from_moments(t, c, np); set_plane(np); }   // S:49 otherwise

@@ -64,7 +64,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
     int* out = part + start;
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
-    const double margin_z = ap.adaptive_seed_selection_margin * states[f].sensor_height;  // S:90
+    // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
+    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[f].sensor_height) : -INFINITY;
 
     RvpfPlanes rv;
     rv.n = 0;
@@ -79,7 +80,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
     // candidate of the LPR selection: alive and, in zone 0, not below the adaptive margin (S:88-96)
     auto lpr_valid = [&](const float4& p) {
       bool v = (rv.n == 0) || is_alive(rv, ap.th_dist_v, p.x, p.y, p.z);
-      if (zone0 && ((double) p.z < margin_z)) v = false;
+      if (p.z < margin_f) v = false;
       return v;
     };
 
@@ -216,11 +217,12 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
       return s_lpr;
     };
 
-    // ---- one pass + plane fit. MODE 0: seeds {alive, z < zthr} (FUSED: also the inner set {z < zin});
+    // ---- one pass + plane fit. MODE 0: seeds {alive, z < zthr} (FUSED: also the inner set {z < zin}; both float_ru of the
+    //      double thresholds);
     //      MODE 1: {alive, signed distance to `cls` < th_dist}. Leaves the counts in nsel[0..1] and, for non-empty
     //      sets, the fitted planes in s_plane / s_plane2 (valid until the next call). ----
     int nsel[2] = {0, 0};
-    auto fit_pass = [&](int mode, bool fused, double zthr, double zin, const Plane& cls, const double cc[3]) {
+    auto fit_pass = [&](int mode, bool fused, float zthr, float zin, const Plane& cls, const double cc[3]) {
       double a[9], b[FUSE ? 9 : 1];
 #pragma unroll
       for (int q = 0; q < 9; ++q) a[q] = 0.0;
@@ -239,7 +241,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
           const float4 p = q[u];
           bool in = j < n;
           if (in && rv.n != 0) in = is_alive(rv, ap.th_dist_v, p.x, p.y, p.z);
-          if (mode == 0) in = in && ((double) p.z < zthr);                                   // S:108 / S:145
+          if (mode == 0) in = in && (p.z < zthr);                                            // S:108 / S:145
           else if (in) {
             int fl = dist_filter(pf, thf, p.x, p.y, p.z);
             if (fl < 0) fl = (point_plane_distance(cls, p.x, p.y, p.z) < ap.th_dist) ? 1 : 0;   // S:525 / S:529, exact
@@ -250,7 +252,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
             a[0] += dx; a[1] += dy; a[2] += dz;
             a[3] += dx * dx; a[4] += dx * dy; a[5] += dx * dz; a[6] += dy * dy; a[7] += dy * dz; a[8] += dz * dz;
             ++na;
-            if (FUSE && fused && ((double) p.z < zin)) {
+            if (FUSE && fused && (p.z < zin)) {
               b[0] += dx; b[1] += dy; b[2] += dz;
               b[3] += dx * dx; b[4] += dx * dy; b[5] += dx * dz; b[6] += dy * dy; b[7] += dy * dz; b[8] += dz * dz;
               ++nb;
@@ -258,23 +260,26 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
           }
         }
       }
-#pragma unroll
-      for (int q = 0; q < 9; ++q) a[q] = warp_sum(a[q]);
+      // warp sums by reduce-scatter (pwpp_fit.cuh): the lane that ends up holding quantity q stores it
       na = __reduce_add_sync(0xffffffffu, na);
       if (FUSE && fused) {
+        double v[18];
 #pragma unroll
-        for (int q = 0; q < (FUSE ? 9 : 1); ++q) b[q] = warp_sum(b[q]);
+        for (int q = 0; q < 9; ++q) { v[q] = a[q]; v[9 + q] = b[FUSE ? q : 0]; }
+        reduce_scatter<18, 16>(v, lane);
+#pragma unroll
+        for (int q = 0; q < 18; ++q)
+          if (lane == rs_lane(18, 16, q)) s_part[w][q] = v[rs_slot(18, 16, q)];
         nb = __reduce_add_sync(0xffffffffu, nb);
+      } else {
+        reduce_scatter<9, 16>(a, lane);
+#pragma unroll
+        for (int q = 0; q < 9; ++q)
+          if (lane == rs_lane(9, 16, q)) s_part[w][q] = a[rs_slot(9, 16, q)];
       }
       if (lane == 0) {
-#pragma unroll
-        for (int q = 0; q < 9; ++q) s_part[w][q] = a[q];
         s_pcnt[w][0] = na;
-        if (FUSE && fused) {
-#pragma unroll
-          for (int q = 0; q < (FUSE ? 9 : 1); ++q) s_part[w][9 + q] = b[q];
-          s_pcnt[w][1] = nb;
-        }
+        if (FUSE && fused) s_pcnt[w][1] = nb;
       }
       __syncthreads();
       if (w == 0) {
@@ -314,7 +319,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
       for (int it = 0; it < ap.num_iter; ++it) {
         const double lpr = select_lpr();
         c[2] = lpr;
-        fit_pass(0, fuse_ok, lpr + ap.th_seeds_v, lpr + ap.th_seeds, pl, c);
+        fit_pass(0, fuse_ok, float_ru(lpr + ap.th_seeds_v), float_ru(lpr + ap.th_seeds), pl, c);
         if (nsel[0] > 0) { pl = s_plane; have_plane = true; }
         if (have_plane && pl.normal[2] < ap.uprightness_thr) {  // S:489
           if (rv.n < MAX_RVPF) rv.pl[rv.n++] = pl;
@@ -331,7 +336,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
     if (!seed_done) {
       const double lpr = select_lpr();
       c[2] = lpr;
-      fit_pass(0, false, lpr + ap.th_seeds, 0.0, pl, c);
+      fit_pass(0, false, float_ru(lpr + ap.th_seeds), 0.f, pl, c);
       if (nsel[0] > 0) { pl = s_plane; have_plane = true; }
     }
     int n_ground = 0;
@@ -339,7 +344,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
       if (!have_plane) break;
       const Plane cls = pl;
       const double cc[3] = {pl.mean[0], pl.mean[1], pl.mean[2]};
-      fit_pass(1, false, 0.0, 0.0, cls, cc);
+      fit_pass(1, false, 0.f, 0.f, cls, cc);
       if (nsel[0] > 0) pl = s_plane;
     }
     // last iteration (S:528-542): split by the current plane, then refit on the ground part
@@ -347,7 +352,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
       const Plane cls = pl;
       {
         const double cc[3] = {pl.mean[0], pl.mean[1], pl.mean[2]};
-        fit_pass(1, false, 0.0, 0.0, cls, cc);
+        fit_pass(1, false, 0.f, 0.f, cls, cc);
         n_ground = nsel[0];
         if (n_ground > 0) pl = s_plane;
       }

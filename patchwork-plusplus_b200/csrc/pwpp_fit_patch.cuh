@@ -60,16 +60,6 @@ __device__ __forceinline__ double rank_mean(const unsigned* cbuf, int cc, int ta
 constexpr int FP_SL = 16;    // points per thread (register slots)
 constexpr int FP_STG = 256;  // staging entries per warp: the participating points of 8 slots
 
-__device__ __forceinline__ float float_ru(double t) {
-#if defined(__CUDA_ARCH__)
-  return __double2float_ru(t);
-#else
-  float f = (float) t;                       // round to nearest, then step up if that went below t
-  if ((double) f < t) f = nextafterf(f, INFINITY);
-  return f;
-#endif
-}
-
 // 9 sums + 2 counts reduced over the warp with all chains in flight (xor butterfly: every lane ends with the totals)
 __device__ __forceinline__ void warp_sum9(double (&a)[9], int& c0, int& c1) {
 #pragma unroll

@@ -79,6 +79,22 @@ PW_HD float fsqrt(float a) {
 #endif
 }
 
+// Smallest float >= t (NaN stays NaN). For every float z, ±inf and NaN included:  (double) z < t  <=>  z < float_ru(t).
+// If float_ru(t) == t both sides compare the same value. Otherwise no float lies in [t, float_ru(t)), so a float is
+// below t exactly when it is below float_ru(t). NaN on either side makes both compares false. The fit kernels compute
+// it once per round, so that the per-point tests against a double threshold are one fp32 compare instead of a
+// float->double conversion (a quarter of the FP64 rate on sm_90) plus a double compare.
+PW_HD float float_ru(double t) {
+  float f = (float) t;   // round to nearest, then step up to the next float if that went below t
+  if ((double) f < t) {  // f is finite or -inf here
+    uint32_t b;
+    memcpy(&b, &f, sizeof b);
+    b = (f == 0.0f) ? 1u : (f > 0.0f ? b + 1u : b - 1u);
+    memcpy(&f, &b, sizeof f);
+  }
+  return f;
+}
+
 #define PW_PI 3.14159265358979323846 /* M_PI, reference patchworkpp.h:4-6 */
 
 // double atan2 of the exact (rare) paths: kept out of line on the device so that the unrolled hot loops of the
