@@ -8,6 +8,14 @@
 //
 //   pwpp_sequence DIR [--device N] [--repeat R] [--quiet]
 // Prints per frame: points, ground, non-ground, patches, adaptive sensor height, call time; then frames/s end to end.
+//
+//   pwpp_sequence DIR [DIR ...] [--frames-per-call K] [--device N] [--repeat R] [--quiet]
+// Several sensors (or one sensor in batches): every directory is one stream of one context, and every call of
+// pwpp_estimate_host_streams carries the next K scans (default 1) of every directory that still has scans, time-major
+// (dir 0 scan t, dir 1 scan t, ..., dir 0 scan t+1, ...). Directories may hold different numbers of scans: a stream
+// that ran out is simply not named any more. Each line is prefixed with the stream (directory) index; the height is the
+// stream's adaptive sensor height after that frame, "-" where the stream has a later frame in the same call (the state
+// between two frames of one call is not kept).
 #include <patchwork/patchworkpp.h>
 
 #include <algorithm>
@@ -20,6 +28,11 @@
 #include <string>
 #include <thread>
 #include <vector>
+
+// The several-streams form calls pwpp_estimate_host_streams. The reference to it is weak, so the runner still links, and its
+// one-directory form still runs, against a C-ABI library that predates the stream table; the several-streams form then
+// says so and exits with 1.
+#pragma weak pwpp_estimate_host_streams
 
 namespace {
 struct Slot {
@@ -62,18 +75,93 @@ bool load(const std::string& path, Slot& s) {
   s.n = (int64_t) (got / 4);
   return true;
 }
+
+// Several directories, one stream each, K scans of every stream per call (see the header comment).
+int run_streams(const std::vector<std::string>& dirs, int frames_per_call, int device, int repeat, bool quiet) {
+  if (!&pwpp_estimate_host_streams) {
+    std::fprintf(stderr, "pwpp_sequence: this libpwpp_b200 has no pwpp_estimate_host_streams (stream table): several directories or "
+                         "--frames-per-call need a newer library\n");
+    return 1;
+  }
+  const int ns = (int) dirs.size();
+  std::vector<std::vector<std::string>> files(ns);
+  size_t longest = 0;
+  for (int d = 0; d < ns; ++d) {
+    const std::vector<std::string> once = list_scans(dirs[d]);
+    if (once.empty()) { std::fprintf(stderr, "no *.bin scans in %s\n", dirs[d].c_str()); return 2; }
+    for (int r = 0; r < repeat; ++r) files[d].insert(files[d].end(), once.begin(), once.end());
+    longest = std::max(longest, files[d].size());
+  }
+  pwpp_params params;
+  pwpp_params_default(&params);   // reference defaults (patchworkpp.h:79-111)
+  pwpp_ctx* ctx = nullptr;
+  if (pwpp_create(&params, device, ns, 0, &ctx) != PWPP_OK) { std::fprintf(stderr, "pwpp_sequence: %s\n", pwpp_last_error()); return 1; }
+  pwpp_set_output_order(ctx, PWPP_ORDER_REFERENCE);   // the order of the single-directory run (the drop-in class)
+  std::vector<Slot> slots;            // one page-locked buffer per frame position of a call
+  std::vector<int32_t> streams;
+  std::vector<const float*> ptrs;
+  std::vector<int64_t> counts;
+  std::vector<int> last_of(ns);
+  const auto t0 = std::chrono::steady_clock::now();
+  long long points = 0;
+  int done = 0, calls = 0, rc = 0;
+  for (size_t t0_scan = 0; t0_scan < longest && rc == 0; t0_scan += (size_t) frames_per_call) {
+    streams.clear(); ptrs.clear(); counts.clear();
+    for (size_t t = t0_scan; t < std::min(longest, t0_scan + (size_t) frames_per_call) && rc == 0; ++t)
+      for (int d = 0; d < ns; ++d) {
+        if (t >= files[d].size()) continue;
+        const size_t f = streams.size();
+        if (slots.size() <= f) slots.resize(f + 1);
+        Slot& s = slots[f];
+        s.name = files[d][t];
+        if (!load(dirs[d] + "/" + s.name, s)) { std::fprintf(stderr, "failed to read %s\n", s.name.c_str()); rc = 1; break; }
+        streams.push_back(d);
+        ptrs.push_back(s.data);
+        counts.push_back(s.n);
+        last_of[d] = (int) f;
+      }
+    if (rc || streams.empty()) break;
+    const int nf = (int) streams.size();
+    if (pwpp_estimate_host_streams(ctx, nf, streams.data(), ptrs.data(), counts.data(), 4, 4, 1) != PWPP_OK) {
+      std::fprintf(stderr, "pwpp_sequence: %s\n", pwpp_last_error());
+      rc = 1;
+      break;
+    }
+    ++calls;
+    for (int f = 0; f < nf && !quiet; ++f) {
+      const int d = streams[f];
+      char height[32] = "-";
+      if (last_of[d] == f) std::snprintf(height, sizeof height, "%.4f", pwpp_height(ctx, d));
+      std::printf("%-3d %-14s points %7lld  ground %7lld  nonground %7lld  patches %4d  height %s  call %.3f ms\n", d, slots[f].name.c_str(),
+                  (long long) counts[f], (long long) pwpp_num_ground(ctx, f), (long long) pwpp_num_nonground(ctx, f), pwpp_num_patches(ctx, f), height,
+                  pwpp_time_us(ctx) / 1000.0);
+    }
+    for (int f = 0; f < nf; ++f) points += counts[f];
+    done += nf;
+  }
+  const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  std::printf("%d frames of %d streams in %d calls, %lld points in %.3f s: %.1f frames/s end to end (disk -> pinned -> GPU -> counts)\n", done, ns, calls,
+              points, sec, done / sec);
+  for (Slot& s : slots) if (s.data) pwpp_host_free(s.data);
+  pwpp_destroy(ctx);
+  return rc;
+}
 }  // namespace
 
 int main(int argc, char** argv) {
-  if (argc < 2) { std::fprintf(stderr, "usage: %s DIR [--device N] [--repeat R] [--quiet]\n", argv[0]); return 2; }
-  const std::string dir = argv[1];
-  int device = 0, repeat = 1;
+  if (argc < 2) { std::fprintf(stderr, "usage: %s DIR [DIR ...] [--frames-per-call K] [--device N] [--repeat R] [--quiet]\n", argv[0]); return 2; }
+  std::vector<std::string> dirs{argv[1]};
+  int device = 0, repeat = 1, frames_per_call = 0;
   bool quiet = false;
   for (int i = 2; i < argc; ++i) {
     if (!std::strcmp(argv[i], "--device") && i + 1 < argc) device = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--repeat") && i + 1 < argc) repeat = std::atoi(argv[++i]);
+    else if (!std::strcmp(argv[i], "--frames-per-call") && i + 1 < argc) frames_per_call = std::atoi(argv[++i]);
     else if (!std::strcmp(argv[i], "--quiet")) quiet = true;
+    else if (std::strncmp(argv[i], "--", 2) != 0) dirs.push_back(argv[i]);
   }
+  if (dirs.size() > 1 || frames_per_call > 0) return run_streams(dirs, std::max(1, frames_per_call), device, std::max(1, repeat), quiet);
+  const std::string dir = dirs[0];
   const std::vector<std::string> files = list_scans(dir);
   if (files.empty()) { std::fprintf(stderr, "no *.bin scans in %s\n", dir.c_str()); return 2; }
   const int total = (int) files.size() * repeat;

@@ -16,9 +16,18 @@
  * Model: a `pwpp_ctx` owns `num_streams` independent sensor streams. One stream is what
  * the reference calls one PatchWorkpp instance (H:114-235): it carries the temporal state
  * (adaptive elevation/flatness thresholds, their histories, the adaptive sensor height —
- * S:338-375) from frame to frame. One call processes ONE frame for each of the first
- * `nframes` streams, all on the GPU, in a single launch sequence. The reference class maps
- * to a ctx with num_streams == 1.
+ * S:338-375) from frame to frame. pwpp_estimate_host / pwpp_estimate_device process ONE frame
+ * for each of the first `nframes` streams, all on the GPU, in a single launch sequence. The
+ * *_streams variants take a stream table instead: frame f of the call belongs to stream
+ * streams[f], any subset of the streams in any order, a stream possibly several times (its
+ * frames then run in call order, see "Stream table" below). The reference class maps to a ctx
+ * with num_streams == 1.
+ *
+ * Indexing rule: everything a call PRODUCES is indexed by the frame's position f in the call
+ * (counts, index lists, xyz, centers, normals, patch records, bin ids, pwpp_device_results,
+ * pwpp_host_results); the temporal STATE is indexed by stream id (pwpp_get_state, pwpp_height,
+ * pwpp_copy_history, pwpp_export_state / pwpp_import_state, pwpp_reset_stream). With the
+ * identity table of pwpp_estimate_host / pwpp_estimate_device the two coincide.
  *
  * All functions returning int return PWPP_OK (0) or a negative pwpp_status; the message
  * for the last failure on the calling thread is available from pwpp_last_error().
@@ -147,12 +156,29 @@ int pwpp_estimate_device(pwpp_ctx* ctx, int nframes, const void* d_pts,
  * S:379-382): the rows are padded to the kernels' 16-byte points by a device-side copy into the ctx's input buffer. */
 int pwpp_estimate_device_xyz(pwpp_ctx* ctx, int nframes, const void* d_xyz, const int64_t* h_offsets, void* cuda_stream);
 
+/* Stream table: the same two paths with frame f of the call belonging to stream streams[f]
+ * (0 <= streams[f] < num_streams; 1 <= nframes <= 65535, nframes may exceed num_streams).
+ *   - Any subset of the streams, in any order. Streams the call does not name keep their state untouched.
+ *   - A stream may appear several times: its frames are processed in call order, each one sees the state the
+ *     previous one left (exactly as in separate calls). The call is split into maximal runs of consecutive
+ *     frames with pairwise distinct streams; each run is one launch sequence over its frames, and stream
+ *     order serialises the runs. In pwpp_estimate_host the launch ranges are its pipeline chunks cut at the
+ *     run boundaries, so the upload of later frames still overlaps the kernels of earlier ones.
+ *   - Results are indexed by call position f, state by stream id (the indexing rule above).
+ *   - A NULL table, an id out of range or nframes outside [1, 65535] returns PWPP_ERR_INVALID_ARG before anything
+ *     is launched: no stream's state changes.
+ * pwpp_estimate_host / pwpp_estimate_device are these with the identity table streams[f] = f. */
+int pwpp_estimate_host_streams(pwpp_ctx* ctx, int nframes, const int32_t* streams, const float* const* pts, const int64_t* n,
+                               int cols, int64_t row_stride, int64_t col_stride);
+int pwpp_estimate_device_streams(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* d_pts, const int64_t* h_offsets,
+                                 int has_intensity, void* cuda_stream);
+
 /* cudaDeviceSynchronize() on the ctx's device: what a binding calls before handing device memory produced on an unknown
  * stream to pwpp_estimate_device (and what makes its results visible to every stream afterwards). */
 int pwpp_device_synchronize(pwpp_ctx* ctx);
 int pwpp_synchronize(pwpp_ctx* ctx);
 
-/* ---- results of the last estimate call, per frame/stream f ------------------------------ */
+/* ---- results of the last estimate call, per frame f (position in the call) -------------- */
 
 /* getGroundIndices / getNongroundIndices (H:159-160, S:18-26): int32 indices into the frame's
  * point array. Every input point appears in exactly one of the two lists (S:545-548).
@@ -172,7 +198,7 @@ int pwpp_copy_nonground_xyz(pwpp_ctx* ctx, int f, float* dst);
 int pwpp_num_patches(pwpp_ctx* ctx, int f);
 int pwpp_copy_centers(pwpp_ctx* ctx, int f, float* dst);
 int pwpp_copy_normals(pwpp_ctx* ctx, int f, float* dst);
-/* getHeight (H:154): the ADAPTIVE sensor height after the last frame (S:348). */
+/* getHeight (H:154): the ADAPTIVE sensor height of STREAM f after its last frame (S:348). */
 double pwpp_height(pwpp_ctx* ctx, int f);
 /* getTimeTaken (H:155): microseconds of the last estimate call (whole call, all frames). */
 double pwpp_time_us(pwpp_ctx* ctx);
@@ -256,7 +282,7 @@ const char* pwpp_stage_name(int stage);
 /* Number of kernels this ctx has launched since creation. */
 int64_t pwpp_launch_count(const pwpp_ctx* ctx);
 
-/* ---- temporal state (S:338-375) ---------------------------------------------------------- */
+/* ---- temporal state (S:338-375), per STREAM f --------------------------------------------- */
 
 int pwpp_get_state(pwpp_ctx* ctx, int f, pwpp_state* out);
 /* Histories: ring r of update_elevation_ / update_flatness_ (H:174-175); dst holds n_* doubles. */

@@ -138,6 +138,7 @@ struct pwpp_ctx {
   DevBuf<float> d_cm;             // host path: column-major frames as uploaded, repacked on the device
   DevBuf<long long> d_pt_off;     // [F+1]
   DevBuf<int> d_chunk_off;        // [F+1]
+  DevBuf<int> d_stream;           // [F] stream of every frame of the call
   DevBuf<unsigned short> d_bin_ids;
   DevBuf<unsigned short> d_chist;
   DevBuf<unsigned int> d_cbase;
@@ -155,16 +156,22 @@ struct pwpp_ctx {
   int max_sectors = 0;
   FitLaunch order_k[ORD_NUM_HEADS];   // k_order_cta<512, X>, <512, L3>, <256, L2>, <128, L1>, k_order_warp (same argument list as the fit kernels' type is not needed: launched by name)
   DevBuf<int> d_out_idx;
-  DevBuf<int> d_counts;           // [3][F]: num_ground, num_patches, num_dropped
+  DevBuf<int> d_counts;           // [3][F]: num_ground, num_patches, num_dropped (F = frames of the call)
   DevBuf<float> d_centers, d_normals;  // [F][nbins][3]
   DevBuf<float> d_xyz;            // gather scratch
 
   PinBuf<float4> h_in;
   PinBuf<long long> h_pt_off_buf[2];      // double-buffered: a call never waits for the previous call's upload
   PinBuf<int> h_chunk_off_buf[2];
+  PinBuf<int> h_stream_buf[2];
   cudaEvent_t tab_ev[2] = {nullptr, nullptr};
   int tab_cur = 0;
   std::vector<int> chunk_off;             // host copy of the current call's chunk table
+  // Frames of one stream are sequentially dependent (k_gle of one frame writes what the next one reads), so a call is
+  // launched as runs of consecutive frames with pairwise distinct streams: frames [runs[r], runs[r + 1]) are run r.
+  std::vector<int> runs;
+  std::vector<int> identity;              // [num_streams] 0, 1, 2, ...: the stream table of pwpp_estimate_host / _device
+  std::vector<int> last_pos;              // [num_streams] scratch of the run split, -1 between calls
   PinBuf<int> h_out_idx;
   PinBuf<int> h_counts;
   PinBuf<float> h_centers, h_normals;
@@ -179,7 +186,7 @@ struct pwpp_ctx {
   cudaStream_t last_stream = nullptr;
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
-  struct GraphKey { int nf, has_intensity, chunks; unsigned long long gen; const void* pts; };
+  struct GraphKey { int nf, call_frames, has_intensity, chunks; unsigned long long gen; const void* pts; };
   cudaGraphExec_t gexec[2] = {nullptr, nullptr};
   GraphKey gkey[2] = {};
   long long glaunches[2] = {0, 0};
@@ -214,17 +221,45 @@ int bind_device(pwpp_ctx* ctx) {
   return PWPP_OK;
 }
 
-// Sizes the work buffers for a call over nframes frames (ctx->pt_off filled) and uploads the frame tables.
-int prepare_call(pwpp_ctx* ctx, int nframes, cudaStream_t s) {
+// Checks the stream table of a call: 1 <= nframes <= 65535 (a grid dimension of the per-frame kernels), every id a stream of
+// the ctx. Nothing is launched and no state changes when it fails.
+int check_streams(const pwpp_ctx* ctx, int nframes, const int32_t* streams) {
+  if (!streams) return fail(PWPP_ERR_INVALID_ARG, "streams is NULL");
+  if (nframes < 1 || nframes > 65535) return fail(PWPP_ERR_INVALID_ARG, "nframes must be in [1, 65535]");
+  for (int f = 0; f < nframes; ++f)
+    if (streams[f] < 0 || streams[f] >= ctx->num_streams)
+      return fail(PWPP_ERR_INVALID_ARG, "stream id " + std::to_string(streams[f]) + " of frame " + std::to_string(f) + " is outside [0, num_streams)");
+  return PWPP_OK;
+}
+
+// Splits a call into maximal runs of consecutive frames whose streams are pairwise distinct (ctx->runs).
+void split_runs(pwpp_ctx* ctx, int nframes, const int32_t* streams) {
+  ctx->runs.assign(1, 0);
+  for (int f = 0; f < nframes; ++f) {
+    int& p = ctx->last_pos[streams[f]];
+    if (p >= ctx->runs.back()) ctx->runs.push_back(f);   // the stream already has a frame in the current run
+    p = f;
+  }
+  ctx->runs.push_back(nframes);
+  for (int f = 0; f < nframes; ++f) ctx->last_pos[streams[f]] = -1;
+}
+
+// Sizes the work buffers for a call over nframes frames (ctx->pt_off filled), uploads the frame tables (points, chunks,
+// stream of every frame) and splits the call into runs.
+int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_t s) {
   const long long total = ctx->pt_off[nframes];
   int total_chunks = 0;
   ctx->tab_cur ^= 1;
   const int tb = ctx->tab_cur;
   PinBuf<long long>& h_pt_off = ctx->h_pt_off_buf[tb];
   PinBuf<int>& h_chunk_off = ctx->h_chunk_off_buf[tb];
+  PinBuf<int>& h_stream = ctx->h_stream_buf[tb];
   CU_TRY(cudaEventSynchronize(ctx->tab_ev[tb]));   // upload issued two calls ago: long finished
   CU_TRY(h_pt_off.reserve(nframes + 1));
   CU_TRY(h_chunk_off.reserve(nframes + 1));
+  CU_TRY(h_stream.reserve(nframes));
+  std::memcpy(h_stream.p, streams, (size_t) nframes * sizeof(int));
+  split_runs(ctx, nframes, streams);
   ctx->chunk_off.assign(nframes + 1, 0);
   for (int f = 0; f < nframes; ++f) {
     const long long n = ctx->pt_off[f + 1] - ctx->pt_off[f];
@@ -240,6 +275,7 @@ int prepare_call(pwpp_ctx* ctx, int nframes, cudaStream_t s) {
   const int nb = ctx->g.nbins, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO;
   CU_TRY(ctx->d_pt_off.reserve(nframes + 1));
   CU_TRY(ctx->d_chunk_off.reserve(nframes + 1));
+  CU_TRY(ctx->d_stream.reserve(nframes));
   CU_TRY(ctx->d_bin_ids.reserve((size_t) total));
   CU_TRY(ctx->d_chist.reserve((size_t) total_chunks * nbp));
   CU_TRY(ctx->d_cbase.reserve((size_t) total_chunks * nbp));
@@ -251,11 +287,12 @@ int prepare_call(pwpp_ctx* ctx, int nframes, cudaStream_t s) {
   CU_TRY(ctx->d_segs.reserve((size_t) nframes * nb_all));
   for (int c = 0; c < NUM_CLASSES; ++c) CU_TRY(ctx->d_wq_items[c].reserve((size_t) nframes * nb));
   CU_TRY(ctx->d_out_idx.reserve((size_t) total));
-  CU_TRY(ctx->d_counts.reserve((size_t) 3 * ctx->num_streams));
+  CU_TRY(ctx->d_counts.reserve((size_t) 3 * nframes));
   CU_TRY(ctx->d_centers.reserve((size_t) nframes * nb * 3));
   CU_TRY(ctx->d_normals.reserve((size_t) nframes * nb * 3));
   CU_TRY(cudaMemcpyAsync(ctx->d_pt_off.p, h_pt_off.p, (nframes + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_chunk_off.p, h_chunk_off.p, (nframes + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+  CU_TRY(cudaMemcpyAsync(ctx->d_stream.p, h_stream.p, nframes * sizeof(int), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaEventRecord(ctx->tab_ev[tb], s));
   ctx->last_nframes = nframes;
   ctx->last_total = total;
@@ -264,18 +301,19 @@ int prepare_call(pwpp_ctx* ctx, int nframes, cudaStream_t s) {
   return PWPP_OK;
 }
 
-// Launches the whole path for frames [f0, f0 + nf) of the prepared call on stream s. A frame range is the same
-// launch sequence over per-frame arrays offset by f0 (frame tables hold absolute point / chunk positions), which is
-// what lets pwpp_estimate_host pipeline chunks of frames against their H2D / D2H copies.
+// Launches the whole path for frames [f0, f0 + nf) of the prepared call on stream s; the range must not hold two frames of
+// one stream (a run or part of one). A frame range is the same launch sequence over per-frame arrays offset by f0 (frame
+// tables hold absolute point / chunk positions), which is what lets pwpp_estimate_host pipeline chunks of frames against
+// their H2D / D2H copies. Stream state and histories are indexed by the stream table, never by the frame.
 int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int has_intensity, cudaStream_t s, bool prof, int chunks_override) {
   int max_chunks = 0;
   for (int f = f0; f < f0 + nf; ++f) max_chunks = std::max(max_chunks, ctx->chunk_off[f + 1] - ctx->chunk_off[f]);
   if (chunks_override > 0) max_chunks = chunks_override;   // graph capture: grids sized for a range of frame sizes (surplus CTAs exit at once)
   const int nb = ctx->g.nbins, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO;
   const int nframes = nf;
-  FrameTable ft{ctx->d_pt_off.p + f0, ctx->d_chunk_off.p + f0};
-  StreamState* states = ctx->d_states.p + f0;
-  double* hist = ctx->d_hist.p + (size_t) f0 * 2 * 4 * ctx->hcap;
+  FrameTable ft{ctx->d_pt_off.p + f0, ctx->d_chunk_off.p + f0, ctx->d_stream.p + f0};
+  StreamState* states = ctx->d_states.p;
+  double* hist = ctx->d_hist.p;
   int* bin_off = ctx->d_bin_off.p + (size_t) f0 * (nbp + 1);
   BinFit* fits = ctx->d_fits.p + (size_t) f0 * nb;
   BinSeg* segs = ctx->d_segs.p + (size_t) f0 * nb_all;
@@ -402,9 +440,10 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
     stage += 6;
   }
 #undef FIT_ARGS
+  const int call_frames = ctx->last_nframes;   // the count rows are as long as the call
   int* d_ng = ctx->d_counts.p + f0;
-  int* d_np = ctx->d_counts.p + ctx->num_streams + f0;
-  int* d_nd = ctx->d_counts.p + 2 * ctx->num_streams + f0;
+  int* d_np = ctx->d_counts.p + call_frames + f0;
+  int* d_nd = ctx->d_counts.p + 2 * call_frames + f0;
   {
     const size_t gle_smem = gle_smem_bytes(ctx->max_sectors);
     k_gle<<<nframes, 32, gle_smem, s>>>(ft, states, hist, ctx->hcap, ctx->g, ctx->ap, nbp, ctx->max_sectors, bin_off, fits, segs, d_ng, d_np, centers, normals, d_nd);
@@ -428,8 +467,9 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
 }
 
 // Small calls are launch-bound (ten kernels of a few microseconds each plus the fork / join events of the fit kernels): the
-// sequence is captured once per (frames, intensity flag, grid size class, buffer generation) and replayed as one CUDA
-// graph. Only for calls whose input sits in the ctx's own upload buffer (the host entry point), so the captured pointers
+// sequence is captured once per (frames, frames of the call, intensity flag, grid size class, buffer generation) and
+// replayed as one CUDA graph; it reads the frame tables (stream ids included) the current call uploaded. Only for the
+// first range of calls whose input sits in the ctx's own upload buffer (the host entry point), so the captured pointers
 // stay valid; PWPP_GRAPH=0 switches it off.
 constexpr int GRAPH_MAX_FRAMES = 16;
 int launch_range(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int has_intensity, cudaStream_t s, bool prof) {
@@ -438,9 +478,10 @@ int launch_range(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int has_int
   for (int f = 0; f < nf; ++f) max_chunks = std::max(max_chunks, ctx->chunk_off[f + 1] - ctx->chunk_off[f]);
   const int capc = std::max(8, (max_chunks + 7) & ~7);
   const int slot = has_intensity ? 1 : 0;
-  const pwpp_ctx::GraphKey key{nf, has_intensity, capc, g_alloc_gen, (const void*) d_pts};
+  const pwpp_ctx::GraphKey key{nf, ctx->last_nframes, has_intensity, capc, g_alloc_gen, (const void*) d_pts};
   pwpp_ctx::GraphKey& have = ctx->gkey[slot];
-  if (!ctx->gexec[slot] || have.nf != key.nf || have.chunks != key.chunks || have.gen != key.gen || have.pts != key.pts) {
+  if (!ctx->gexec[slot] || have.nf != key.nf || have.call_frames != key.call_frames || have.chunks != key.chunks || have.gen != key.gen ||
+      have.pts != key.pts) {
     if (ctx->gexec[slot]) { cudaGraphExecDestroy(ctx->gexec[slot]); ctx->gexec[slot] = nullptr; }
     const long long l0 = ctx->launches;
     CU_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
@@ -478,16 +519,32 @@ long long subbatch_points() {
   return v;
 }
 
-int run_path(pwpp_ctx* ctx, int nframes, const float4* d_pts, int has_intensity, cudaStream_t s) {
-  int rc = prepare_call(ctx, nframes, s);
+// Launches the frames [f0, f1) of the prepared call: one range per run they overlap (stream order serialises the runs).
+// *r is the first run that may overlap; calls with increasing f0 pass the same cursor.
+int launch_runs(pwpp_ctx* ctx, int f0, int f1, size_t* r, const float4* d_pts, int has_intensity, cudaStream_t s, bool prof) {
+  const std::vector<int>& runs = ctx->runs;
+  while (*r + 2 < runs.size() && runs[*r + 1] <= f0) ++*r;
+  for (size_t q = *r; q + 1 < runs.size() && runs[q] < f1; ++q) {
+    const int a = std::max(f0, runs[q]), b = std::min(f1, runs[q + 1]);
+    if (a >= b) continue;
+    const int rc = launch_range(ctx, a, b - a, d_pts, has_intensity, s, prof);
+    if (rc) return rc;
+  }
+  return PWPP_OK;
+}
+
+int run_path(pwpp_ctx* ctx, int nframes, const int32_t* streams, const float4* d_pts, int has_intensity, cudaStream_t s) {
+  int rc = prepare_call(ctx, nframes, streams, s);
   if (rc) return rc;
-  if (ctx->profiling) return launch_range(ctx, 0, nframes, d_pts, has_intensity, s, true);
+  size_t r = 0;
+  // per-stage timing covers one launch sequence: a call of several runs is launched, but not timed
+  if (ctx->profiling) return launch_runs(ctx, 0, nframes, &r, d_pts, has_intensity, s, ctx->runs.size() == 2);
   const long long cap = subbatch_points();
   int f0 = 0;
   while (f0 < nframes) {
     int f1 = f0 + 1;
     while (f1 < nframes && ctx->pt_off[f1 + 1] - ctx->pt_off[f0] <= cap) ++f1;
-    rc = launch_range(ctx, f0, f1 - f0, d_pts, has_intensity, s, false);
+    rc = launch_runs(ctx, f0, f1, &r, d_pts, has_intensity, s, false);
     if (rc) return rc;
     f0 = f1;
   }
@@ -504,8 +561,8 @@ int fetch_counts(pwpp_ctx* ctx) {
   if (ctx->counts_fetched) return PWPP_OK;
   int rc = bind_device(ctx);
   if (rc) return rc;
-  CU_TRY(ctx->h_counts.reserve((size_t) 3 * ctx->num_streams));
-  CU_TRY(cudaMemcpyAsync(ctx->h_counts.p, ctx->d_counts.p, (size_t) 3 * ctx->num_streams * sizeof(int), cudaMemcpyDeviceToHost, ctx->last_stream));
+  CU_TRY(ctx->h_counts.reserve((size_t) 3 * ctx->last_nframes));
+  CU_TRY(cudaMemcpyAsync(ctx->h_counts.p, ctx->d_counts.p, (size_t) 3 * ctx->last_nframes * sizeof(int), cudaMemcpyDeviceToHost, ctx->last_stream));
   CU_TRY(cudaStreamSynchronize(ctx->last_stream));
   ctx->counts_fetched = true;
   return PWPP_OK;
@@ -536,6 +593,8 @@ int fetch_patches(pwpp_ctx* ctx) {
 }
 
 inline int frame_n(const pwpp_ctx* ctx, int f) { return (int) (ctx->pt_off[f + 1] - ctx->pt_off[f]); }
+// fetched count of frame f: q = 0 ground points, 1 patches, 2 dropped points
+inline int count_of(const pwpp_ctx* ctx, int q, int f) { return ctx->h_counts.p[(size_t) q * ctx->last_nframes + f]; }
 
 }  // namespace
 
@@ -576,6 +635,9 @@ int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t 
   ctx->prm = *params;
   ctx->device = device;
   ctx->num_streams = num_streams;
+  ctx->identity.resize(num_streams);
+  for (int i = 0; i < num_streams; ++i) ctx->identity[i] = i;
+  ctx->last_pos.assign(num_streams, -1);
   build_geometry(*params, ctx->g, ctx->ap, ctx->fast_bin);
   ctx->sw_serial_fit = env_int("PWPP_SERIAL_FIT", 0, 0, 1) != 0;       // diagnostic: the fit kernels one after another on the call's stream
   ctx->sw_front = env_int("PWPP_FRONT", PWPP_FRONT_DEFAULT, 0, 1);        // 1: cluster-per-frame front end, 0: k_bin_hist + k_bin_scan + k_scatter
@@ -715,12 +777,14 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   for (int i = 0; i < 2; ++i) if (ctx->tab_ev[i]) cudaEventDestroy(ctx->tab_ev[i]);
   for (int q = 0; q < NUM_SIDE; ++q) { if (ctx->ev_fit[q]) cudaEventDestroy(ctx->ev_fit[q]); if (ctx->ev_join[q]) cudaEventDestroy(ctx->ev_join[q]); if (ctx->side[q]) cudaStreamDestroy(ctx->side[q]); }
   ctx->d_states.release(); ctx->d_states_init.release(); ctx->d_hist.release(); ctx->d_in.release(); ctx->d_cm.release(); ctx->d_pt_off.release(); ctx->d_chunk_off.release();
+  ctx->d_stream.release();
   ctx->d_bin_ids.release(); ctx->d_chist.release(); ctx->d_cbase.release(); ctx->d_bin_off.release(); ctx->d_sorted.release();
   ctx->d_part.release(); ctx->d_labels.release(); ctx->d_fits.release(); ctx->d_segs.release(); ctx->d_wq_ctr.release();
   for (int c = 0; c < NUM_CLASSES; ++c) ctx->d_wq_items[c].release();
   ctx->d_out_idx.release(); ctx->d_counts.release();
   ctx->d_centers.release(); ctx->d_normals.release(); ctx->d_xyz.release();
-  ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); } ctx->h_out_idx.release(); ctx->h_counts.release();
+  ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); }
+  ctx->h_out_idx.release(); ctx->h_counts.release();
   ctx->h_centers.release(); ctx->h_normals.release();
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -777,18 +841,18 @@ const char* pwpp_stage_name(int stage) {
 }
 int64_t pwpp_launch_count(const pwpp_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
-int pwpp_estimate_host(pwpp_ctx* ctx, int nframes, const float* const* pts, const int64_t* n, int cols, int64_t row_stride, int64_t col_stride) {
-  if (!ctx || !pts || !n) return fail(PWPP_ERR_INVALID_ARG, "NULL argument");
-  if (nframes < 1 || nframes > ctx->num_streams) return fail(PWPP_ERR_INVALID_ARG, "nframes must be in [1, num_streams]");
+// The host path of pwpp_estimate_host and pwpp_estimate_host_streams (stream table checked by the caller).
+static int estimate_host_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, const float* const* pts, const int64_t* n, int cols,
+                              int64_t row_stride, int64_t col_stride) {
+  if (!pts || !n) return fail(PWPP_ERR_INVALID_ARG, "NULL argument");
   if (cols != 3 && cols != 4) return fail(PWPP_ERR_INVALID_ARG, "cols must be 3 or 4 (x,y,z[,intensity])");
+  for (int f = 0; f < nframes; ++f)
+    if (n[f] < 0 || (n[f] > 0 && !pts[f])) return fail(PWPP_ERR_INVALID_ARG, "bad frame pointer/size");
   int rc = bind_device(ctx);
   if (rc) return rc;
   const auto t0 = std::chrono::steady_clock::now();
   ctx->pt_off.assign(nframes + 1, 0);
-  for (int f = 0; f < nframes; ++f) {
-    if (n[f] < 0 || (n[f] > 0 && !pts[f])) return fail(PWPP_ERR_INVALID_ARG, "bad frame pointer/size");
-    ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
-  }
+  for (int f = 0; f < nframes; ++f) ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
   const long long total = ctx->pt_off[nframes];
   CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(total, 1)));
   cudaStream_t s = ctx->stream, s_in = ctx->stream_h2d, s_out = ctx->stream_d2h;
@@ -798,10 +862,10 @@ int pwpp_estimate_host(pwpp_ctx* ctx, int nframes, const float* const* pts, cons
   CU_TRY(cudaStreamSynchronize(s));
   CU_TRY(cudaStreamSynchronize(s_in));
   CU_TRY(cudaStreamSynchronize(s_out));
-  rc = prepare_call(ctx, nframes, s);
+  rc = prepare_call(ctx, nframes, streams, s);
   if (rc) return rc;
   CU_TRY(ctx->h_out_idx.reserve((size_t) std::max<long long>(total, 1)));
-  CU_TRY(ctx->h_counts.reserve((size_t) 3 * ctx->num_streams));
+  CU_TRY(ctx->h_counts.reserve((size_t) 3 * nframes));
   const bool packed = (cols == 4 && col_stride == 1 && row_stride == 4);
   bool staged_any = false;
   // Chunks of frames flow through three streams: H2D of chunk k+1 | kernels of chunk k | D2H of chunk k-1.
@@ -816,6 +880,9 @@ int pwpp_estimate_host(pwpp_ctx* ctx, int nframes, const float* const* pts, cons
   // on the critical path of a one-frame call) and four events bracket its three phases (pwpp_call_times_us)
   const bool one_stream = (nchunks == 1);
   if (one_stream) { s_in = s; s_out = s; CU_TRY(cudaEventRecord(ctx->ev_begin, s)); }
+  // the launch ranges are the pipeline chunks cut at the run boundaries; per-stage timing needs one range per call
+  const bool prof = ctx->profiling && nchunks == 1 && ctx->runs.size() == 2;
+  size_t run_cursor = 0;
   for (int k = 0; k < nchunks; ++k) {
     const int f0 = k * chunk_frames, f1 = std::min(nframes, f0 + chunk_frames);
     for (int f = f0; f < f1; ++f) {
@@ -861,16 +928,16 @@ int pwpp_estimate_host(pwpp_ctx* ctx, int nframes, const float* const* pts, cons
     }
     CU_TRY(cudaEventRecord(ctx->ev0, s_in));
     if (!one_stream) CU_TRY(cudaStreamWaitEvent(s, ctx->ev0, 0));
-    rc = launch_range(ctx, f0, f1 - f0, ctx->d_in.p, cols == 4 ? 1 : 0, s, ctx->profiling && nchunks == 1);
+    rc = launch_runs(ctx, f0, f1, &run_cursor, ctx->d_in.p, cols == 4 ? 1 : 0, s, prof);
     if (rc) return rc;
     CU_TRY(cudaEventRecord(ctx->ev1, s));
     if (!one_stream) CU_TRY(cudaStreamWaitEvent(s_out, ctx->ev1, 0));
     const long long o0 = ctx->pt_off[f0], o1 = ctx->pt_off[f1];
-    if (f0 == 0 && f1 == ctx->num_streams) {   // the three count rows are one contiguous block when the chunk covers every stream
-      CU_TRY(cudaMemcpyAsync(ctx->h_counts.p, ctx->d_counts.p, (size_t) 3 * ctx->num_streams * sizeof(int), cudaMemcpyDeviceToHost, s_out));
+    if (f0 == 0 && f1 == nframes) {   // the three count rows are one contiguous block when the chunk covers the whole call
+      CU_TRY(cudaMemcpyAsync(ctx->h_counts.p, ctx->d_counts.p, (size_t) 3 * nframes * sizeof(int), cudaMemcpyDeviceToHost, s_out));
     } else {
       for (int q = 0; q < 3; ++q)
-        CU_TRY(cudaMemcpyAsync(ctx->h_counts.p + (size_t) q * ctx->num_streams + f0, ctx->d_counts.p + (size_t) q * ctx->num_streams + f0,
+        CU_TRY(cudaMemcpyAsync(ctx->h_counts.p + (size_t) q * nframes + f0, ctx->d_counts.p + (size_t) q * nframes + f0,
                                (size_t) (f1 - f0) * sizeof(int), cudaMemcpyDeviceToHost, s_out));
     }
     if (o1 > o0) CU_TRY(cudaMemcpyAsync(ctx->h_out_idx.p + o0, ctx->d_out_idx.p + o0, (size_t) (o1 - o0) * sizeof(int), cudaMemcpyDeviceToHost, s_out));
@@ -885,26 +952,54 @@ int pwpp_estimate_host(pwpp_ctx* ctx, int nframes, const float* const* pts, cons
   return PWPP_OK;
 }
 
-int pwpp_estimate_device(pwpp_ctx* ctx, int nframes, const void* d_pts, const int64_t* h_offsets, int has_intensity, void* cuda_stream) {
-  if (!ctx || !h_offsets) return fail(PWPP_ERR_INVALID_ARG, "NULL argument");
+int pwpp_estimate_host(pwpp_ctx* ctx, int nframes, const float* const* pts, const int64_t* n, int cols, int64_t row_stride, int64_t col_stride) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "NULL argument");
   if (nframes < 1 || nframes > ctx->num_streams) return fail(PWPP_ERR_INVALID_ARG, "nframes must be in [1, num_streams]");
+  return estimate_host_impl(ctx, nframes, ctx->identity.data(), pts, n, cols, row_stride, col_stride);
+}
+
+int pwpp_estimate_host_streams(pwpp_ctx* ctx, int nframes, const int32_t* streams, const float* const* pts, const int64_t* n, int cols,
+                               int64_t row_stride, int64_t col_stride) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  const int rc = check_streams(ctx, nframes, streams);
+  if (rc) return rc;
+  return estimate_host_impl(ctx, nframes, streams, pts, n, cols, row_stride, col_stride);
+}
+
+// The device path of pwpp_estimate_device and pwpp_estimate_device_streams (stream table checked by the caller).
+static int estimate_device_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* d_pts, const int64_t* h_offsets, int has_intensity,
+                                void* cuda_stream) {
+  if (!h_offsets) return fail(PWPP_ERR_INVALID_ARG, "NULL argument");
+  for (int f = 1; f <= nframes; ++f)
+    if (h_offsets[f] < h_offsets[f - 1]) return fail(PWPP_ERR_INVALID_ARG, "offsets must be non-decreasing");
+  if (h_offsets[nframes] > h_offsets[0] && !d_pts) return fail(PWPP_ERR_INVALID_ARG, "d_pts is NULL");
   int rc = bind_device(ctx);
   if (rc) return rc;
   const auto t0 = std::chrono::steady_clock::now();
   ctx->pt_off.assign(nframes + 1, 0);
-  for (int f = 0; f <= nframes; ++f) {
-    ctx->pt_off[f] = h_offsets[f] - h_offsets[0];
-    if (f > 0 && ctx->pt_off[f] < ctx->pt_off[f - 1]) return fail(PWPP_ERR_INVALID_ARG, "offsets must be non-decreasing");
-  }
-  if (ctx->pt_off[nframes] > 0 && !d_pts) return fail(PWPP_ERR_INVALID_ARG, "d_pts is NULL");
+  for (int f = 0; f <= nframes; ++f) ctx->pt_off[f] = h_offsets[f] - h_offsets[0];
   cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
   // work buffers are reused stream-ordered: a call on a different stream than the previous one waits for it
   if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
   if (!ctx->last_stream && s != ctx->stream) CU_TRY(cudaStreamSynchronize(ctx->stream));   // resets issued before the first call ran on the ctx's own stream
-  rc = run_path(ctx, nframes, (const float4*) d_pts + h_offsets[0], has_intensity, s);
+  rc = run_path(ctx, nframes, streams, (const float4*) d_pts + h_offsets[0], has_intensity, s);
   if (rc) return rc;
   ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
   return PWPP_OK;
+}
+
+int pwpp_estimate_device(pwpp_ctx* ctx, int nframes, const void* d_pts, const int64_t* h_offsets, int has_intensity, void* cuda_stream) {
+  if (!ctx || !h_offsets) return fail(PWPP_ERR_INVALID_ARG, "NULL argument");
+  if (nframes < 1 || nframes > ctx->num_streams) return fail(PWPP_ERR_INVALID_ARG, "nframes must be in [1, num_streams]");
+  return estimate_device_impl(ctx, nframes, ctx->identity.data(), d_pts, h_offsets, has_intensity, cuda_stream);
+}
+
+int pwpp_estimate_device_streams(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* d_pts, const int64_t* h_offsets, int has_intensity,
+                                 void* cuda_stream) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  const int rc = check_streams(ctx, nframes, streams);
+  if (rc) return rc;
+  return estimate_device_impl(ctx, nframes, streams, d_pts, h_offsets, has_intensity, cuda_stream);
 }
 
 int pwpp_estimate_device_xyz(pwpp_ctx* ctx, int nframes, const void* d_xyz, const int64_t* h_offsets, void* cuda_stream) {
@@ -949,7 +1044,7 @@ int64_t pwpp_num_ground(pwpp_ctx* ctx, int f) {
 }
 int64_t pwpp_num_nonground(pwpp_ctx* ctx, int f) {
   if (check_frame(ctx, f) || fetch_counts(ctx)) return -1;
-  return (int64_t) frame_n(ctx, f) - ctx->h_counts.p[f] - ctx->h_counts.p[2 * ctx->num_streams + f];
+  return (int64_t) frame_n(ctx, f) - ctx->h_counts.p[f] - count_of(ctx, 2, f);
 }
 int pwpp_copy_ground_indices(pwpp_ctx* ctx, int f, int32_t* dst) {
   int rc = check_frame(ctx, f);
@@ -966,7 +1061,7 @@ int pwpp_copy_nonground_indices(pwpp_ctx* ctx, int f, int32_t* dst) {
   rc = fetch_indices(ctx);
   if (rc) return rc;
   const int ng = ctx->h_counts.p[f];
-  const int nn = frame_n(ctx, f) - ng - ctx->h_counts.p[2 * ctx->num_streams + f];
+  const int nn = frame_n(ctx, f) - ng - count_of(ctx, 2, f);
   if (nn > 0) std::memcpy(dst, ctx->h_out_idx.p + ctx->pt_off[f] + ng, (size_t) nn * sizeof(int32_t));
   return PWPP_OK;
 }
@@ -977,7 +1072,7 @@ static int copy_xyz(pwpp_ctx* ctx, int f, float* dst, bool ground) {
   rc = fetch_counts(ctx);
   if (rc) return rc;
   const int ng = ctx->h_counts.p[f];
-  const int nn = frame_n(ctx, f) - ng - ctx->h_counts.p[2 * ctx->num_streams + f];
+  const int nn = frame_n(ctx, f) - ng - count_of(ctx, 2, f);
   const int cnt = ground ? ng : nn;
   if (cnt <= 0) return PWPP_OK;
   CU_TRY(ctx->d_xyz.reserve((size_t) cnt * 3));
@@ -993,14 +1088,14 @@ int pwpp_copy_nonground_xyz(pwpp_ctx* ctx, int f, float* dst) { return copy_xyz(
 
 int pwpp_num_patches(pwpp_ctx* ctx, int f) {
   if (check_frame(ctx, f) || fetch_counts(ctx)) return -1;
-  return ctx->h_counts.p[ctx->num_streams + f];
+  return count_of(ctx, 1, f);
 }
 int pwpp_copy_centers(pwpp_ctx* ctx, int f, float* dst) {
   int rc = check_frame(ctx, f);
   if (rc) return rc;
   rc = fetch_patches(ctx);
   if (rc) return rc;
-  const int k = ctx->h_counts.p[ctx->num_streams + f];
+  const int k = count_of(ctx, 1, f);
   if (k > 0) std::memcpy(dst, ctx->h_centers.p + (size_t) f * ctx->g.nbins * 3, (size_t) k * 3 * sizeof(float));
   return PWPP_OK;
 }
@@ -1009,7 +1104,7 @@ int pwpp_copy_normals(pwpp_ctx* ctx, int f, float* dst) {
   if (rc) return rc;
   rc = fetch_patches(ctx);
   if (rc) return rc;
-  const int k = ctx->h_counts.p[ctx->num_streams + f];
+  const int k = count_of(ctx, 1, f);
   if (k > 0) std::memcpy(dst, ctx->h_normals.p + (size_t) f * ctx->g.nbins * 3, (size_t) k * 3 * sizeof(float));
   return PWPP_OK;
 }

@@ -14,9 +14,28 @@ constexpr int WARP_ITERS = WARP_PTS / 32;                   // 16
 constexpr int MAX_LPR = 64;          // num_lpr supported by the warp selection buffer
 constexpr int MAX_RVPF = 8;          // num_iter supported (R-VPF planes kept in registers)
 
+#if defined(PWPP_SIMT_EMU)
+// tests/simt (the kernels run on the CPU): the stream table of a FrameTable whose initializer names none. It is the identity
+// table (frame f -> stream f, what the twin's multi-frame calls mean) unless a harness points it at another table for the
+// duration of a call. Device builds have no default: pwpp_capi.cu always passes the call's table.
+inline const int* simt_identity_streams() {
+  static int v[65536];
+  static const bool filled = [] { for (int i = 0; i < 65536; ++i) v[i] = i; return true; }();
+  (void) filled;
+  return v;
+}
+inline const int* g_simt_streams = simt_identity_streams();
+#endif
+
 struct FrameTable {            // per call, device arrays indexed by frame
   const long long* pt_off;     // [F+1] first point of each frame in the packed point array
   const int* chunk_off;        // [F+1] first chunk of each frame
+  // [F] stream of each frame: index of its StreamState and of its history rows
+#if defined(PWPP_SIMT_EMU)
+  const int* stream = g_simt_streams;
+#else
+  const int* stream;
+#endif
 };
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }

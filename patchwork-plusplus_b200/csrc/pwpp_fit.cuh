@@ -256,7 +256,7 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
     // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
-    const float margin_f = (have && zone0) ? float_ru(ap.adaptive_seed_selection_margin * states[f].sensor_height) : -INFINITY;
+    const float margin_f = (have && zone0) ? float_ru(ap.adaptive_seed_selection_margin * states[ft.stream[f]].sensor_height) : -INFINITY;
     double c0x = 0.0, c0y = 0.0;               // first point: reference point of the shifted moments of the seed fits
     if (have) { const float4 p = P[0]; c0x = (double) p.x; c0y = (double) p.y; }
 
@@ -509,7 +509,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
     // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
-    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[f].sensor_height) : -INFINITY;
+    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[ft.stream[f]].sensor_height) : -INFINITY;
     const float4 first = P[0];
     const double c0x = (double) first.x, c0y = (double) first.y;
 
@@ -1185,7 +1185,7 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
     // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
-    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[f].sensor_height) : -INFINITY;
+    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[ft.stream[f]].sensor_height) : -INFINITY;
     const float4 first = P[0];
     double c[3] = {(double) first.x, (double) first.y, 0.0};   // reference point of all moment sums of this patch
 

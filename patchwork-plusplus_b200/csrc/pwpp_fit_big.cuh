@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
     // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
-    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[f].sensor_height) : -INFINITY;
+    const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[ft.stream[f]].sensor_height) : -INFINITY;
 
     RvpfPlanes rv;
     rv.n = 0;

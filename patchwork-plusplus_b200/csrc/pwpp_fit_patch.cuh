@@ -161,7 +161,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_patch(const float4* __res
     }
     PW_EV(2);
     const bool zone0 = bin < g.bin_base[1];
-    const double margin_z = ap.adaptive_seed_selection_margin * states[f].sensor_height;   // S:90
+    const double margin_z = ap.adaptive_seed_selection_margin * states[ft.stream[f]].sensor_height;   // S:90
     const float margin_f = zone0 ? float_ru(margin_z) : -INFINITY;                          // (double) z < margin  <=>  z < margin_f
     if (tid == 0) { s_first[0] = px[0]; s_first[1] = py[0]; }   // point 0: reference point of the moment sums (with the LPR height); read after the first barrier of the seed round
     double c0 = 0.0, c1 = 0.0;

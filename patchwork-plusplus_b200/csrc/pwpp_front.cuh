@@ -70,7 +70,7 @@ __launch_bounds__(NT, 1024 / NT) k_front_cluster(const float4* __restrict__ pts,
   const int i0 = (int) ((long long) nrows * gw / (FC_CS * FC_WARPS)) << 5;                        // this warp's points [i0, i1)
   const int i1 = min(n, (int) ((long long) nrows * (gw + 1) / (FC_CS * FC_WARPS)) << 5);
   const float4* fp = pts + p0;
-  const double sensor_height = states[f].sensor_height;
+  const double sensor_height = states[ft.stream[f]].sensor_height;
   const bool rnr_on = ap.enable_RNR && has_intensity;  // S:161, S:379-382
   unsigned* my = s_wb + (size_t) w * nbp;
   float4* my_tile = s_tile + (size_t) w * 2 * FC_CHUNK;

@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(CHUNK_THREADS, 4) k_bin_hist(const float4* __r
   if ((int) blockIdx.x >= nchunks) return;
   for (int b = threadIdx.x; b < nbp; b += CHUNK_THREADS) s_hist[b] = 0;
   __syncthreads();
-  const double sensor_height = states[f].sensor_height;
+  const double sensor_height = states[ft.stream[f]].sensor_height;
   const bool rnr_on = ap.enable_RNR && has_intensity;  // S:161, S:379-382
   const int warp = threadIdx.x >> 5, lane = lane_id();
   const int base = blockIdx.x * CHUNK_PTS + warp * WARP_PTS;
@@ -290,15 +290,16 @@ __global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restri
   const int f = blockIdx.x;
   const int lane = lane_id();
   const unsigned lt = lanemask_lt();
-  StreamState& st = states[f];
+  const int sid = ft.stream[f];                       // frame f of the call advances stream sid
+  StreamState& st = states[sid];
   const int nb = g.nbins, nb_all = nb + PW_NUM_PSEUDO;
   const int* bo = bin_off + (size_t) f * (nbp + 1);
   BinFit* fit = fits + (size_t) f * nb;
   BinSeg* seg = segs + (size_t) f * nb_all;
   float* cen = centers + (size_t) f * nb * 3;
   float* nor = normals + (size_t) f * nb * 3;
-  double* h_elev = hist + ((size_t) f * 2 + 0) * 4 * hcap;
-  double* h_flat = hist + ((size_t) f * 2 + 1) * 4 * hcap;
+  double* h_elev = hist + ((size_t) sid * 2 + 0) * 4 * hcap;
+  double* h_flat = hist + ((size_t) sid * 2 + 1) * 4 * hcap;
 
 #if !defined(PWPP_SIMT_EMU)
   // The ring loop below is a chain of ~20 dependent round trips to this frame's patch records (104 B each, written by the fit

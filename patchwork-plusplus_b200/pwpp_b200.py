@@ -34,6 +34,9 @@ def load_library():
     lib.pwpp_num_bins.argtypes = [vp]; lib.pwpp_num_bins.restype = i32
     lib.pwpp_estimate_host.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(i64), i32, i64, i64]; lib.pwpp_estimate_host.restype = i32
     lib.pwpp_estimate_device.argtypes = [vp, i32, vp, C.POINTER(i64), i32, vp]; lib.pwpp_estimate_device.restype = i32
+    lib.pwpp_estimate_host_streams.argtypes = [vp, i32, vp, C.POINTER(vp), C.POINTER(i64), i32, i64, i64]
+    lib.pwpp_estimate_host_streams.restype = i32
+    lib.pwpp_estimate_device_streams.argtypes = [vp, i32, vp, vp, C.POINTER(i64), i32, vp]; lib.pwpp_estimate_device_streams.restype = i32
     lib.pwpp_synchronize.argtypes = [vp]; lib.pwpp_synchronize.restype = i32
     for n in ("pwpp_num_ground", "pwpp_num_nonground"):
         getattr(lib, n).argtypes = [vp, i32]; getattr(lib, n).restype = i64
@@ -108,16 +111,29 @@ class Engine:
             pass
 
     # ---- hot path ----
-    def estimate_host(self, frames):
-        """frames: list of C-contiguous float32 arrays (n_f, 3|4), one per stream."""
+    @staticmethod
+    def _stream_table(streams, nf):
+        ids = np.ascontiguousarray(streams, dtype=np.int32)
+        if ids.shape != (nf,):
+            raise PwppError(f"streams must name one stream per frame ({nf}), got shape {ids.shape}")
+        return ids
+
+    def estimate_host(self, frames, streams=None):
+        """frames: list of C-contiguous float32 arrays (n_f, 3|4). Without `streams` frame f goes to stream f; with it, to
+        stream streams[f] (any subset, any order, repeats run in call order). Results are indexed by the frame's position
+        in the call, state by stream id."""
         frames = [np.ascontiguousarray(f, dtype=np.float32) for f in frames]
         cols = frames[0].shape[1]
         assert all(f.ndim == 2 and f.shape[1] == cols for f in frames)
         nf = len(frames)
         ptrs = (C.c_void_p * nf)(*[f.ctypes.data for f in frames])
         ns = (C.c_int64 * nf)(*[f.shape[0] for f in frames])
+        if streams is None:
+            _check(self.lib.pwpp_estimate_host(self._h, nf, ptrs, ns, cols, cols, 1))
+        else:
+            ids = self._stream_table(streams, nf)
+            _check(self.lib.pwpp_estimate_host_streams(self._h, nf, ids.ctypes.data, ptrs, ns, cols, cols, 1))
         self._n = [f.shape[0] for f in frames]
-        _check(self.lib.pwpp_estimate_host(self._h, nf, ptrs, ns, cols, cols, 1))
 
     def estimate_host_strided(self, ptrs, ns, cols, row_stride, col_stride):
         nf = len(ptrs)
@@ -126,12 +142,18 @@ class Engine:
         self._n = list(ns)
         _check(self.lib.pwpp_estimate_host(self._h, nf, p, n, cols, row_stride, col_stride))
 
-    def estimate_device(self, d_ptr: int, offsets, has_intensity: bool = True, stream: int = 0):
+    def estimate_device(self, d_ptr: int, offsets, has_intensity: bool = True, stream: int = 0, streams=None):
+        """Packed float4 points on the device, frame f at [offsets[f], offsets[f + 1]); `streams` as for estimate_host."""
         offsets = np.ascontiguousarray(offsets, dtype=np.int64)
         nf = len(offsets) - 1
+        offs = offsets.ctypes.data_as(C.POINTER(C.c_int64))
+        if streams is None:
+            _check(self.lib.pwpp_estimate_device(self._h, nf, C.c_void_p(d_ptr), offs, 1 if has_intensity else 0, C.c_void_p(stream)))
+        else:
+            ids = self._stream_table(streams, nf)
+            _check(self.lib.pwpp_estimate_device_streams(self._h, nf, ids.ctypes.data, C.c_void_p(d_ptr), offs, 1 if has_intensity else 0,
+                                                         C.c_void_p(stream)))
         self._n = np.diff(offsets).tolist()
-        _check(self.lib.pwpp_estimate_device(self._h, nf, C.c_void_p(d_ptr), offsets.ctypes.data_as(C.POINTER(C.c_int64)),
-                                             1 if has_intensity else 0, C.c_void_p(stream)))
 
     def synchronize(self):
         _check(self.lib.pwpp_synchronize(self._h))
