@@ -27,7 +27,9 @@
  * (counts, index lists, xyz, centers, normals, patch records, bin ids, pwpp_device_results,
  * pwpp_host_results); the temporal STATE is indexed by stream id (pwpp_get_state, pwpp_height,
  * pwpp_copy_history, pwpp_export_state / pwpp_import_state, pwpp_reset_stream). With the
- * identity table of pwpp_estimate_host / pwpp_estimate_device the two coincide.
+ * identity table of pwpp_estimate_host / pwpp_estimate_device the two coincide. The PARAMETERS a frame
+ * runs with are those of its stream's set (pwpp_create_sets; one set for a ctx from pwpp_create): results
+ * by call position, state by stream id, parameters by the stream's set.
  *
  * All functions returning int return PWPP_OK (0) or a negative pwpp_status; the message
  * for the last failure on the calling thread is available from pwpp_last_error().
@@ -46,6 +48,7 @@ extern "C" {
 #define PWPP_ABI_VERSION 1
 #define PWPP_NUM_ZONES 4            /* H:127-134 hard-wires 4 zones via .at(0..3)          */
 #define PWPP_MAX_RINGS_OF_INTEREST 4 /* H:174-175: update_flatness_[4], update_elevation_[4] */
+#define PWPP_MAX_PARAM_SETS 8       /* parameter sets of one ctx (pwpp_create_sets) */
 
 typedef enum pwpp_status {
   PWPP_OK = 0,
@@ -123,12 +126,28 @@ typedef struct pwpp_ctx pwpp_ctx;
  * capacity grows on demand if a later call exceeds it. */
 int pwpp_create(const pwpp_params* params, int device, int num_streams,
                 int64_t max_points_per_frame, pwpp_ctx** out);
+
+/* Several parameter sets in one ctx: stream s runs with sets[stream_set[s]] for its whole life, exactly like a
+ * reference instance constructed with those Params (H:120), and one call may mix streams of any sets. Per-frame
+ * results follow the frame's set: pwpp_copy_bin_results writes that set's nbins records, pwpp_copy_bin_ids uses its
+ * pseudo-bin ids (nbins, nbins + 1), centers / normals / patch counts cover its bins. State follows the stream's set:
+ * reset restores the set's sensor_height / elevation_thr / flatness_thr, the history bound (hist_cap, see pwpp_state)
+ * is the set's own, and a stream's state blob is the one a one-set ctx with that set produces (importable either way).
+ * Every set goes through the checks of pwpp_create; num_sets must be in [1, PWPP_MAX_PARAM_SETS] and stream_set a
+ * non-NULL array of num_streams ids in [0, num_sets). A failure returns PWPP_ERR_INVALID_ARG or PWPP_ERR_UNSUPPORTED
+ * (the message names the set) before anything is allocated. pwpp_create is this with one set. */
+int pwpp_create_sets(const pwpp_params* sets, int num_sets, const int32_t* stream_set, int device, int num_streams,
+                     int64_t max_points_per_frame, pwpp_ctx** out);
 void pwpp_destroy(pwpp_ctx* ctx);
 
 const char* pwpp_last_error(void);
 int pwpp_abi_version(void);
-/* Number of polar bins of the configured concentric-zone model (504 with defaults). */
+/* Number of polar bins of the configured concentric-zone model (504 with defaults). With several parameter sets: the
+ * largest bin count of the sets (a pwpp_copy_bin_results buffer of that size fits any frame). */
 int pwpp_num_bins(const pwpp_ctx* ctx);
+/* Bin count of stream s's parameter set, and the set id of stream s (negative status for a bad s). */
+int pwpp_stream_num_bins(const pwpp_ctx* ctx, int s);
+int pwpp_stream_set(const pwpp_ctx* ctx, int s);
 
 /* ---- the hot path ---------------------------------------------------------------------- */
 
@@ -260,7 +279,7 @@ typedef struct pwpp_bin_result {
 #define PWPP_VERDICT_TGR_REVERTED 5   /* S:444-450 */
 #define PWPP_VERDICT_TGR_REJECTED 6   /* S:452-458, or enable_TGR == false (S:297-299) */
 
-int pwpp_copy_bin_results(pwpp_ctx* ctx, int f, pwpp_bin_result* dst /* [pwpp_num_bins] */);
+int pwpp_copy_bin_results(pwpp_ctx* ctx, int f, pwpp_bin_result* dst /* [nbins of frame f's set, <= pwpp_num_bins] */);
 /* Polar bin id of every point of frame f as computed by the binning kernel:
  * 0..nbins-1, or nbins (= RNR hit, S:391-396) or nbins+1 (= outside (min_range,max_range], S:617-619). */
 int pwpp_copy_bin_ids(pwpp_ctx* ctx, int f, uint16_t* dst /* [n_f] */);
@@ -293,7 +312,8 @@ int pwpp_copy_history(pwpp_ctx* ctx, int f, int ring, int which /*0=elevation,1=
  * opaque blob. A blob exported from stream f of one ctx can be imported into any stream of any ctx created with the
  * same parameters (another GPU, another process, a later run): the next frame then gives bit-identical results.
  * pwpp_export_state synchronizes with the last estimate call; pwpp_import_state takes effect before the next one. */
-size_t pwpp_state_blob_size(const pwpp_ctx* ctx);
+size_t pwpp_state_blob_size(const pwpp_ctx* ctx);           /* the largest over the sets: fits any stream's blob */
+size_t pwpp_stream_state_blob_size(const pwpp_ctx* ctx, int s); /* the blob of stream s (its set's hist_cap); 0 for a bad s */
 int pwpp_export_state(pwpp_ctx* ctx, int f, void* blob /* [pwpp_state_blob_size] */);
 int pwpp_import_state(pwpp_ctx* ctx, int f, const void* blob, size_t bytes);
 /* Re-initialises stream f / all streams to the constructor state (a fresh PatchWorkpp instance).

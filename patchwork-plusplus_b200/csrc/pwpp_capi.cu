@@ -98,7 +98,7 @@ __global__ void k_pad_xyz(const float* __restrict__ src, long long n, float4* __
   if (i < n) dst[i] = make_float4(src[3 * i], src[3 * i + 1], src[3 * i + 2], 0.f);
 }
 
-typedef void (*FitKernel)(const float4*, FrameTable, const StreamState*, Geometry, AlgoParams, int, const int*, WorkQueues, int*, BinFit*);
+typedef void (*FitKernel)(const float4*, FrameTable, const StreamState*, GeometrySets, AlgoParamSets, int, const int*, WorkQueues, int*, BinFit*);
 struct FitLaunch {
   FitKernel fn = nullptr;
   int grid = 0, threads = 0;
@@ -108,14 +108,17 @@ struct FitLaunch {
 constexpr int NUM_SIDE = 6;
 
 struct pwpp_ctx {
-  pwpp_params prm;
-  Geometry g;
-  AlgoParams ap;
+  // parameter sets (pwpp_create: one) and the set of every stream; the kernels get the set records by value
+  int num_sets = 1;
+  GeometrySets gs;                          // gs.nbs: the largest bin count of the sets, stride of the per-frame bin arrays
+  AlgoParamSets aps;
+  bool set_fast[MAX_PARAM_SETS] = {};       // build_geometry: the fp32 binning filter is exact for the set's geometry
+  int set_hcap[MAX_PARAM_SETS] = {};        // history row capacity of the set (history_cap)
+  std::vector<int> stream_set;              // [num_streams]
   int device = 0;
   int num_streams = 0;
-  int nbp = 0;      // padded number of bins incl. pseudo-bins
-  int hcap = 0;     // history row capacity (doubles)
-  bool fast_bin = true;
+  int nbp = 0;          // padded number of bins incl. pseudo-bins, of the set with the most bins
+  int hist_stride = 0;  // row stride of d_hist in doubles: the largest set_hcap
   // kernel-variant switches, read from the environment when the context is created (see pwpp_create)
   int sw_front = 1, sw_patch = 0, small_call_frames = 0;
   bool sw_serial_fit = false, front_dense_ok = false;
@@ -139,6 +142,7 @@ struct pwpp_ctx {
   DevBuf<long long> d_pt_off;     // [F+1]
   DevBuf<int> d_chunk_off;        // [F+1]
   DevBuf<int> d_stream;           // [F] stream of every frame of the call
+  DevBuf<int> d_pset;             // [F] parameter set of every frame of the call
   DevBuf<unsigned short> d_bin_ids;
   DevBuf<unsigned short> d_chist;
   DevBuf<unsigned int> d_cbase;
@@ -164,9 +168,11 @@ struct pwpp_ctx {
   PinBuf<long long> h_pt_off_buf[2];      // double-buffered: a call never waits for the previous call's upload
   PinBuf<int> h_chunk_off_buf[2];
   PinBuf<int> h_stream_buf[2];
+  PinBuf<int> h_pset_buf[2];
   cudaEvent_t tab_ev[2] = {nullptr, nullptr};
   int tab_cur = 0;
   std::vector<int> chunk_off;             // host copy of the current call's chunk table
+  std::vector<int> frame_set;             // host copy of the current call's set table
   // Frames of one stream are sequentially dependent (k_gle of one frame writes what the next one reads), so a call is
   // launched as runs of consecutive frames with pairwise distinct streams: frames [runs[r], runs[r + 1]) are run r.
   std::vector<int> runs;
@@ -186,7 +192,7 @@ struct pwpp_ctx {
   cudaStream_t last_stream = nullptr;
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
-  struct GraphKey { int nf, call_frames, has_intensity, chunks; unsigned long long gen; const void* pts; };
+  struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
   cudaGraphExec_t gexec[2] = {nullptr, nullptr};
   GraphKey gkey[2] = {};
   long long glaunches[2] = {0, 0};
@@ -214,6 +220,18 @@ int validate_params(const pwpp_params* p) {
   }
   if (nb + PW_NUM_PSEUDO > 4096) return fail(PWPP_ERR_UNSUPPORTED, "more than 4093 bins are not supported");
   return PWPP_OK;
+}
+
+// The dynamic shared-memory limit is an attribute of the kernel, shared by every context of the process: a context only ever
+// raises it, so that a context whose geometry needs less (fewer bins, fewer sectors) does not break the launches of one that
+// needs more.
+template <typename F>
+cudaError_t raise_smem_limit(F* fn, size_t bytes) {
+  cudaFuncAttributes a;
+  const cudaError_t e = cudaFuncGetAttributes(&a, (const void*) fn);
+  if (e != cudaSuccess) return e;
+  if ((size_t) a.maxDynamicSharedSizeBytes >= bytes) return cudaSuccess;
+  return cudaFuncSetAttribute((const void*) fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bytes);
 }
 
 int bind_device(pwpp_ctx* ctx) {
@@ -254,11 +272,15 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   PinBuf<long long>& h_pt_off = ctx->h_pt_off_buf[tb];
   PinBuf<int>& h_chunk_off = ctx->h_chunk_off_buf[tb];
   PinBuf<int>& h_stream = ctx->h_stream_buf[tb];
+  PinBuf<int>& h_pset = ctx->h_pset_buf[tb];
   CU_TRY(cudaEventSynchronize(ctx->tab_ev[tb]));   // upload issued two calls ago: long finished
   CU_TRY(h_pt_off.reserve(nframes + 1));
   CU_TRY(h_chunk_off.reserve(nframes + 1));
   CU_TRY(h_stream.reserve(nframes));
+  CU_TRY(h_pset.reserve(nframes));
   std::memcpy(h_stream.p, streams, (size_t) nframes * sizeof(int));
+  ctx->frame_set.resize(nframes);
+  for (int f = 0; f < nframes; ++f) h_pset.p[f] = ctx->frame_set[f] = ctx->stream_set[streams[f]];
   split_runs(ctx, nframes, streams);
   ctx->chunk_off.assign(nframes + 1, 0);
   for (int f = 0; f < nframes; ++f) {
@@ -272,10 +294,11 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   h_pt_off.p[nframes] = total;
   h_chunk_off.p[nframes] = total_chunks;
   ctx->chunk_off[nframes] = total_chunks;
-  const int nb = ctx->g.nbins, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO;
+  const int nb = ctx->gs.nbs, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO;
   CU_TRY(ctx->d_pt_off.reserve(nframes + 1));
   CU_TRY(ctx->d_chunk_off.reserve(nframes + 1));
   CU_TRY(ctx->d_stream.reserve(nframes));
+  CU_TRY(ctx->d_pset.reserve(nframes));
   CU_TRY(ctx->d_bin_ids.reserve((size_t) total));
   CU_TRY(ctx->d_chist.reserve((size_t) total_chunks * nbp));
   CU_TRY(ctx->d_cbase.reserve((size_t) total_chunks * nbp));
@@ -293,12 +316,21 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   CU_TRY(cudaMemcpyAsync(ctx->d_pt_off.p, h_pt_off.p, (nframes + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_chunk_off.p, h_chunk_off.p, (nframes + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_stream.p, h_stream.p, nframes * sizeof(int), cudaMemcpyHostToDevice, s));
+  CU_TRY(cudaMemcpyAsync(ctx->d_pset.p, h_pset.p, nframes * sizeof(int), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaEventRecord(ctx->tab_ev[tb], s));
   ctx->last_nframes = nframes;
   ctx->last_total = total;
   ctx->counts_fetched = ctx->idx_fetched = ctx->patches_fetched = false;
   ctx->stage_valid = false;
   return PWPP_OK;
+}
+
+// The fp32 binning filter is used for a launch range only when build_geometry allows it for every set the range names;
+// otherwise the range takes the exact kernel. Both bin exactly, so the bins are the same either way.
+bool range_fast(const pwpp_ctx* ctx, int f0, int nf) {
+  for (int f = f0; f < f0 + nf; ++f)
+    if (!ctx->set_fast[ctx->frame_set[f]]) return false;
+  return true;
 }
 
 // Launches the whole path for frames [f0, f0 + nf) of the prepared call on stream s; the range must not hold two frames of
@@ -309,9 +341,10 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
   int max_chunks = 0;
   for (int f = f0; f < f0 + nf; ++f) max_chunks = std::max(max_chunks, ctx->chunk_off[f + 1] - ctx->chunk_off[f]);
   if (chunks_override > 0) max_chunks = chunks_override;   // graph capture: grids sized for a range of frame sizes (surplus CTAs exit at once)
-  const int nb = ctx->g.nbins, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO;
+  const int nb = ctx->gs.nbs, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO;   // strides of the per-frame bin arrays (the largest set)
   const int nframes = nf;
-  FrameTable ft{ctx->d_pt_off.p + f0, ctx->d_chunk_off.p + f0, ctx->d_stream.p + f0};
+  FrameTable ft{ctx->d_pt_off.p + f0, ctx->d_chunk_off.p + f0, ctx->d_stream.p + f0, ctx->d_pset.p + f0};
+  const bool fast = range_fast(ctx, f0, nf);
   StreamState* states = ctx->d_states.p;
   double* hist = ctx->d_hist.p;
   int* bin_off = ctx->d_bin_off.p + (size_t) f0 * (nbp + 1);
@@ -343,12 +376,12 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
       const int nt = dense ? FC_THREADS_DENSE : FC_THREADS;
       const size_t sm_f = front_cluster_smem_bytes(nbp, nt);
       dim3 grid(FC_CS, nframes);
-#define FC_ARGS d_pts, ft, states, ctx->g, ctx->ap, has_intensity, nbp, nb, ctx->d_bin_ids.p, bin_off, wq, fits, ctx->d_sorted.p
+#define FC_ARGS d_pts, ft, states, ctx->gs, ctx->aps, has_intensity, nbp, nb, ctx->d_bin_ids.p, bin_off, wq, fits, ctx->d_sorted.p
       if (dense) {
-        if (ctx->fast_bin) k_front_cluster<true, CLS_L2_MAX, FC_THREADS_DENSE><<<grid, nt, sm_f, s>>>(FC_ARGS);
+        if (fast) k_front_cluster<true, CLS_L2_MAX, FC_THREADS_DENSE><<<grid, nt, sm_f, s>>>(FC_ARGS);
         else k_front_cluster<false, CLS_L2_MAX, FC_THREADS_DENSE><<<grid, nt, sm_f, s>>>(FC_ARGS);
       } else {
-        if (ctx->fast_bin) k_front_cluster<true, CLS_L2_MAX, FC_THREADS><<<grid, nt, sm_f, s>>>(FC_ARGS);
+        if (fast) k_front_cluster<true, CLS_L2_MAX, FC_THREADS><<<grid, nt, sm_f, s>>>(FC_ARGS);
         else k_front_cluster<false, CLS_L2_MAX, FC_THREADS><<<grid, nt, sm_f, s>>>(FC_ARGS);
       }
 #undef FC_ARGS
@@ -360,14 +393,14 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
     if (max_chunks > 0) {
       dim3 grid(max_chunks, nframes);
       const size_t sm_h = nbp * sizeof(unsigned int);
-#define HIST_ARGS d_pts, ft, states, ctx->g, ctx->ap, has_intensity, nbp, ctx->d_bin_ids.p, ctx->d_chist.p
-      if (!ctx->fast_bin) k_bin_hist<false, 0><<<grid, CHUNK_THREADS, sm_h, s>>>(HIST_ARGS);
+#define HIST_ARGS d_pts, ft, states, ctx->gs, ctx->aps, has_intensity, nbp, ctx->d_bin_ids.p, ctx->d_chist.p
+      if (!fast) k_bin_hist<false, 0><<<grid, CHUNK_THREADS, sm_h, s>>>(HIST_ARGS);
       else k_bin_hist<true, 2><<<grid, CHUNK_THREADS, sm_h, s>>>(HIST_ARGS);
 #undef HIST_ARGS
       ++ctx->launches;
     }
     STAGE_MARK();
-    k_bin_scan<CLS_L2_MAX><<<nframes, 512, (nbp + 1) * sizeof(int), s>>>(ft, nbp, nb, ctx->ap.num_min_pts, ctx->d_chist.p, ctx->d_cbase.p, bin_off, wq, fits);
+    k_bin_scan<CLS_L2_MAX><<<nframes, 512, (nbp + 1) * sizeof(int), s>>>(ft, nbp, nb, ctx->gs, ctx->aps, ctx->d_chist.p, ctx->d_cbase.p, bin_off, wq, fits);
     ++ctx->launches;
     STAGE_MARK();
     if (max_chunks > 0) {
@@ -381,7 +414,7 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
   // persistent fit kernels, one per patch-size class (queues were filled by k_bin_scan). The classes are independent:
   // unless per-stage timing is requested they run on side streams so that the tail of one class (few long patches
   // left) overlaps the start of the next.
-#define FIT_ARGS ctx->d_sorted.p, ft, states, ctx->g, ctx->ap, nbp, bin_off, wq, ctx->d_part.p, fits
+#define FIT_ARGS ctx->d_sorted.p, ft, states, ctx->gs, ctx->aps, nbp, bin_off, wq, ctx->d_part.p, fits
   const bool serial_fit = ctx->sw_serial_fit;   // PWPP_SERIAL_FIT: diagnostic switch
   // persistent grids are sized for a full GPU; a small call (one frame per call is the reference's pattern) would launch hundreds
   // of CTAs per class that find their queue empty and, worse, keep the six classes from running side by side: cap the grid
@@ -446,7 +479,7 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
   int* d_nd = ctx->d_counts.p + 2 * call_frames + f0;
   {
     const size_t gle_smem = gle_smem_bytes(ctx->max_sectors);
-    k_gle<<<nframes, 32, gle_smem, s>>>(ft, states, hist, ctx->hcap, ctx->g, ctx->ap, nbp, ctx->max_sectors, bin_off, fits, segs, d_ng, d_np, centers, normals, d_nd);
+    k_gle<<<nframes, 32, gle_smem, s>>>(ft, states, hist, ctx->hist_stride, ctx->gs, ctx->aps, nbp, ctx->max_sectors, bin_off, fits, segs, d_ng, d_np, centers, normals, d_nd);
     ++ctx->launches;
   }
   STAGE_MARK();
@@ -454,7 +487,7 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
   if (max_chunks > 0) {
     const long long max_pts = (long long) max_chunks * CHUNK_PTS;   // upper bound of the largest frame of the range
     dim3 grid((unsigned) ((max_pts + (long long) EMIT_TILE * EMIT_WARPS - 1) / ((long long) EMIT_TILE * EMIT_WARPS)), nframes);
-    k_emit<<<grid, EMIT_WARPS * 32, 0, s>>>(ft, ctx->g, nbp, bin_off, fits, segs, ctx->d_part.p, ctx->d_sorted.p, ctx->d_out_idx.p);
+    k_emit<<<grid, EMIT_WARPS * 32, 0, s>>>(ft, ctx->gs, nbp, bin_off, fits, segs, ctx->d_part.p, ctx->d_sorted.p, ctx->d_out_idx.p);
     ++ctx->launches;
   }
   STAGE_MARK();
@@ -467,8 +500,8 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
 }
 
 // Small calls are launch-bound (ten kernels of a few microseconds each plus the fork / join events of the fit kernels): the
-// sequence is captured once per (frames, frames of the call, intensity flag, grid size class, buffer generation) and
-// replayed as one CUDA graph; it reads the frame tables (stream ids included) the current call uploaded. Only for the
+// sequence is captured once per (frames, frames of the call, intensity flag, grid size class, binning kernel, buffer generation)
+// and replayed as one CUDA graph; it reads the frame tables (stream and set ids included) the current call uploaded. Only for the
 // first range of calls whose input sits in the ctx's own upload buffer (the host entry point), so the captured pointers
 // stay valid; PWPP_GRAPH=0 switches it off.
 constexpr int GRAPH_MAX_FRAMES = 16;
@@ -478,9 +511,9 @@ int launch_range(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int has_int
   for (int f = 0; f < nf; ++f) max_chunks = std::max(max_chunks, ctx->chunk_off[f + 1] - ctx->chunk_off[f]);
   const int capc = std::max(8, (max_chunks + 7) & ~7);
   const int slot = has_intensity ? 1 : 0;
-  const pwpp_ctx::GraphKey key{nf, ctx->last_nframes, has_intensity, capc, g_alloc_gen, (const void*) d_pts};
+  const pwpp_ctx::GraphKey key{nf, ctx->last_nframes, has_intensity, capc, range_fast(ctx, 0, nf) ? 1 : 0, g_alloc_gen, (const void*) d_pts};
   pwpp_ctx::GraphKey& have = ctx->gkey[slot];
-  if (!ctx->gexec[slot] || have.nf != key.nf || have.call_frames != key.call_frames || have.chunks != key.chunks || have.gen != key.gen ||
+  if (!ctx->gexec[slot] || have.nf != key.nf || have.call_frames != key.call_frames || have.chunks != key.chunks || have.fast != key.fast || have.gen != key.gen ||
       have.pts != key.pts) {
     if (ctx->gexec[slot]) { cudaGraphExecDestroy(ctx->gexec[slot]); ctx->gexec[slot] = nullptr; }
     const long long l0 = ctx->launches;
@@ -582,7 +615,7 @@ int fetch_patches(pwpp_ctx* ctx) {
   if (ctx->patches_fetched) return PWPP_OK;
   int rc = fetch_counts(ctx);
   if (rc) return rc;
-  const size_t n = (size_t) ctx->last_nframes * ctx->g.nbins * 3;
+  const size_t n = (size_t) ctx->last_nframes * ctx->gs.nbs * 3;
   CU_TRY(ctx->h_centers.reserve(n));
   CU_TRY(ctx->h_normals.reserve(n));
   CU_TRY(cudaMemcpyAsync(ctx->h_centers.p, ctx->d_centers.p, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->last_stream));
@@ -616,15 +649,20 @@ void pwpp_params_default(pwpp_params* p) {
 
 const char* pwpp_last_error(void) { return g_last_error.c_str(); }
 int pwpp_abi_version(void) { return PWPP_ABI_VERSION; }
-int pwpp_num_bins(const pwpp_ctx* ctx) { return ctx ? ctx->g.nbins : 0; }
+int pwpp_num_bins(const pwpp_ctx* ctx) { return ctx ? ctx->gs.nbs : 0; }
+int pwpp_stream_num_bins(const pwpp_ctx* ctx, int s) {
+  if (!ctx || s < 0 || s >= ctx->num_streams) return fail(PWPP_ERR_INVALID_ARG, "bad stream index");
+  return ctx->gs.g[ctx->stream_set[s]].nbins;
+}
+int pwpp_stream_set(const pwpp_ctx* ctx, int s) {
+  if (!ctx || s < 0 || s >= ctx->num_streams) return fail(PWPP_ERR_INVALID_ARG, "bad stream index");
+  return ctx->stream_set[s];
+}
 
-int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t max_points_per_frame, pwpp_ctx** out) {
-  if (!out) return fail(PWPP_ERR_INVALID_ARG, "out is NULL");
-  *out = nullptr;
-  int rc = validate_params(params);
-  if (rc) return rc;
-  if (num_streams < 1 || num_streams > 65535) return fail(PWPP_ERR_INVALID_ARG, "num_streams must be in [1,65535]");
-  if (max_points_per_frame < 0) return fail(PWPP_ERR_INVALID_ARG, "max_points_per_frame < 0");
+// The context of pwpp_create and pwpp_create_sets: sets and stream_set (NULL: every stream on set 0) are validated.
+static int create_impl(const pwpp_params* sets, int num_sets, const int32_t* stream_set, int device, int num_streams, int64_t max_points_per_frame,
+                       pwpp_ctx** out) {
+  int rc = PWPP_OK;
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev == 0)
@@ -632,22 +670,29 @@ int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t 
                                         "); this library has no CPU path");
   if (device < 0 || device >= ndev) return fail(PWPP_ERR_INVALID_ARG, "device index out of range");
   pwpp_ctx* ctx = new pwpp_ctx();
-  ctx->prm = *params;
   ctx->device = device;
   ctx->num_streams = num_streams;
   ctx->identity.resize(num_streams);
   for (int i = 0; i < num_streams; ++i) ctx->identity[i] = i;
   ctx->last_pos.assign(num_streams, -1);
-  build_geometry(*params, ctx->g, ctx->ap, ctx->fast_bin);
+  ctx->stream_set.assign(num_streams, 0);
+  if (stream_set) ctx->stream_set.assign(stream_set, stream_set + num_streams);
+  ctx->num_sets = num_sets;
+  ctx->gs.nbs = 0;
+  int max_sectors = 0;
+  for (int k = 0; k < num_sets; ++k) {
+    build_geometry(sets[k], ctx->gs.g[k], ctx->aps.a[k], ctx->set_fast[k]);
+    ctx->set_hcap[k] = history_cap(ctx->gs.g[k], ctx->aps.a[k]);
+    ctx->gs.nbs = std::max(ctx->gs.nbs, ctx->gs.g[k].nbins);
+    ctx->hist_stride = std::max(ctx->hist_stride, ctx->set_hcap[k]);
+    for (int z = 0; z < 4; ++z) max_sectors = std::max(max_sectors, ctx->gs.g[k].num_sectors[z]);
+  }
   ctx->sw_serial_fit = env_int("PWPP_SERIAL_FIT", 0, 0, 1) != 0;       // diagnostic: the fit kernels one after another on the call's stream
   ctx->sw_front = env_int("PWPP_FRONT", PWPP_FRONT_DEFAULT, 0, 1);        // 1: cluster-per-frame front end, 0: k_bin_hist + k_bin_scan + k_scatter
   ctx->sw_patch = env_int("PWPP_FIT_PATCH", PWPP_FIT_PATCH_DEFAULT, 0, 1);   // 1: patches above 512 points on k_fit_patch
   ctx->sw_graph = env_int("PWPP_GRAPH", 1, 0, 1);
   ctx->small_call_frames = env_int("PWPP_SMALL_CALL", PWPP_SMALL_CALL_DEFAULT, 0, 64);   // calls of at most this many frames take the small-call kernels (0: never)
-  ctx->nbp = ((ctx->g.nbins + PW_NUM_PSEUDO + 31) / 32) * 32;
-  int max_sectors = 0;
-  for (int k = 0; k < 4; ++k) max_sectors = std::max(max_sectors, ctx->g.num_sectors[k]);
-  ctx->hcap = std::max(params->max_elevation_storage, params->max_flatness_storage) + 4 * max_sectors + 64;
+  ctx->nbp = ((ctx->gs.nbs + PW_NUM_PSEUDO + 31) / 32) * 32;
   ctx->max_sectors = max_sectors;
 #define CU_TRY_CTX(expr)                                                                                  \
   do {                                                                                                    \
@@ -678,10 +723,10 @@ int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t 
   CU_TRY_CTX(ctx->d_states_init.reserve(num_streams));
   {
     std::vector<StreamState> v(num_streams);
-    for (auto& st : v) init_state(*params, st);
+    for (int i = 0; i < num_streams; ++i) init_state(sets[ctx->stream_set[i]], v[i]);   // the constructor state of the stream's set
     CU_TRY_CTX(cudaMemcpy(ctx->d_states_init.p, v.data(), v.size() * sizeof(StreamState), cudaMemcpyHostToDevice));
   }
-  CU_TRY_CTX(ctx->d_hist.reserve((size_t) num_streams * 2 * 4 * ctx->hcap));
+  CU_TRY_CTX(ctx->d_hist.reserve((size_t) num_streams * 2 * 4 * ctx->hist_stride));
   CU_TRY_CTX(ctx->d_counts.reserve((size_t) 3 * num_streams));
   CU_TRY_CTX(ctx->d_wq_ctr.reserve(2 * NUM_CLASSES + ORD_NUM_HEADS));
   {
@@ -715,7 +760,7 @@ int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t 
     ctx->fit_small[4] = {k_fit_patch<16, 1, 4>, 0, 16 * 32, (size_t) 16 * FP_STG * sizeof(float4)};
     for (int c = 0; c < 2 * NUM_CLASSES; ++c) {
       FitLaunch& k = c < NUM_CLASSES ? ctx->fit[c] : ctx->fit_small[c - NUM_CLASSES];
-      if (k.smem > 0) CU_TRY_CTX(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) k.smem));
+      if (k.smem > 0) CU_TRY_CTX(raise_smem_limit(k.fn, k.smem));
       int per_sm = 1;
       CU_TRY_CTX(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, k.threads, k.smem));
       k.grid = std::max(1, per_sm) * prop.multiProcessorCount;
@@ -726,7 +771,7 @@ int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t 
       const int th[ORD_NUM_HEADS] = {512, 512, 256, 128, ORD_WARP_THREADS};
       for (int q = 0; q < ORD_NUM_HEADS; ++q) {
         const size_t sm = q < 4 ? ord_cta_smem_bytes(th[q]) : 0;
-        if (sm > 48 * 1024) CU_TRY_CTX(cudaFuncSetAttribute(fn[q], cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sm));
+        if (sm > 48 * 1024) CU_TRY_CTX(raise_smem_limit(fn[q], sm));
         int per_sm = 1;
         CU_TRY_CTX(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn[q], th[q], sm));
         ctx->order_k[q].grid = std::max(1, per_sm) * prop.multiProcessorCount;
@@ -735,20 +780,20 @@ int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t 
       }
     }
     const size_t gle_smem = gle_smem_bytes(max_sectors);
-    if (gle_smem > 48 * 1024) CU_TRY_CTX(cudaFuncSetAttribute(k_gle, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) gle_smem));
+    if (gle_smem > 48 * 1024) CU_TRY_CTX(raise_smem_limit(k_gle, gle_smem));
   }
   {
     const size_t scat = (size_t) (CHUNK_THREADS / 32) * ctx->nbp * sizeof(unsigned int);
-    if (scat > 48 * 1024) CU_TRY_CTX(cudaFuncSetAttribute(k_scatter<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) scat));
+    if (scat > 48 * 1024) CU_TRY_CTX(raise_smem_limit(k_scatter<false, 4>, scat));
     const size_t sm_f = front_cluster_smem_bytes(ctx->nbp, FC_THREADS), sm_fd = front_cluster_smem_bytes(ctx->nbp, FC_THREADS_DENSE);
     if (sm_f > 220 * 1024) ctx->sw_front = 0;   // (thousands of bins: the per-warp count tables no longer fit next to the tiles)
     ctx->front_dense_ok = sm_fd <= 220 * 1024;
     if (ctx->sw_front) {
-      CU_TRY_CTX(cudaFuncSetAttribute(k_front_cluster<true, CLS_L2_MAX, FC_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sm_f));
-      CU_TRY_CTX(cudaFuncSetAttribute(k_front_cluster<false, CLS_L2_MAX, FC_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sm_f));
+      CU_TRY_CTX(raise_smem_limit(k_front_cluster<true, CLS_L2_MAX, FC_THREADS>, sm_f));
+      CU_TRY_CTX(raise_smem_limit(k_front_cluster<false, CLS_L2_MAX, FC_THREADS>, sm_f));
       if (ctx->front_dense_ok) {
-        CU_TRY_CTX(cudaFuncSetAttribute(k_front_cluster<true, CLS_L2_MAX, FC_THREADS_DENSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sm_fd));
-        CU_TRY_CTX(cudaFuncSetAttribute(k_front_cluster<false, CLS_L2_MAX, FC_THREADS_DENSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sm_fd));
+        CU_TRY_CTX(raise_smem_limit(k_front_cluster<true, CLS_L2_MAX, FC_THREADS_DENSE>, sm_fd));
+        CU_TRY_CTX(raise_smem_limit(k_front_cluster<false, CLS_L2_MAX, FC_THREADS_DENSE>, sm_fd));
       }
     }
   }
@@ -767,6 +812,44 @@ int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t 
   return PWPP_OK;
 }
 
+static int check_create_args(int num_streams, int64_t max_points_per_frame, pwpp_ctx** out) {
+  if (!out) return fail(PWPP_ERR_INVALID_ARG, "out is NULL");
+  *out = nullptr;
+  if (num_streams < 1 || num_streams > 65535) return fail(PWPP_ERR_INVALID_ARG, "num_streams must be in [1,65535]");
+  if (max_points_per_frame < 0) return fail(PWPP_ERR_INVALID_ARG, "max_points_per_frame < 0");
+  return PWPP_OK;
+}
+
+int pwpp_create(const pwpp_params* params, int device, int num_streams, int64_t max_points_per_frame, pwpp_ctx** out) {
+  if (!out) return fail(PWPP_ERR_INVALID_ARG, "out is NULL");
+  *out = nullptr;
+  int rc = validate_params(params);
+  if (rc) return rc;
+  rc = check_create_args(num_streams, max_points_per_frame, out);
+  if (rc) return rc;
+  return create_impl(params, 1, nullptr, device, num_streams, max_points_per_frame, out);
+}
+
+int pwpp_create_sets(const pwpp_params* sets, int num_sets, const int32_t* stream_set, int device, int num_streams, int64_t max_points_per_frame,
+                     pwpp_ctx** out) {
+  if (!out) return fail(PWPP_ERR_INVALID_ARG, "out is NULL");
+  *out = nullptr;
+  if (num_sets < 1 || num_sets > PWPP_MAX_PARAM_SETS)
+    return fail(PWPP_ERR_INVALID_ARG, "num_sets must be in [1, " + std::to_string(PWPP_MAX_PARAM_SETS) + "], got " + std::to_string(num_sets));
+  if (!sets) return fail(PWPP_ERR_INVALID_ARG, "sets is NULL");
+  for (int k = 0; k < num_sets; ++k) {
+    const int rc = validate_params(&sets[k]);
+    if (rc) return fail(rc, "parameter set " + std::to_string(k) + ": " + g_last_error);
+  }
+  int rc = check_create_args(num_streams, max_points_per_frame, out);
+  if (rc) return rc;
+  if (!stream_set) return fail(PWPP_ERR_INVALID_ARG, "stream_set is NULL");
+  for (int i = 0; i < num_streams; ++i)
+    if (stream_set[i] < 0 || stream_set[i] >= num_sets)
+      return fail(PWPP_ERR_INVALID_ARG, "stream " + std::to_string(i) + " names parameter set " + std::to_string(stream_set[i]) + ", outside [0, num_sets)");
+  return create_impl(sets, num_sets, stream_set, device, num_streams, max_points_per_frame, out);
+}
+
 void pwpp_destroy(pwpp_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
@@ -777,13 +860,13 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   for (int i = 0; i < 2; ++i) if (ctx->tab_ev[i]) cudaEventDestroy(ctx->tab_ev[i]);
   for (int q = 0; q < NUM_SIDE; ++q) { if (ctx->ev_fit[q]) cudaEventDestroy(ctx->ev_fit[q]); if (ctx->ev_join[q]) cudaEventDestroy(ctx->ev_join[q]); if (ctx->side[q]) cudaStreamDestroy(ctx->side[q]); }
   ctx->d_states.release(); ctx->d_states_init.release(); ctx->d_hist.release(); ctx->d_in.release(); ctx->d_cm.release(); ctx->d_pt_off.release(); ctx->d_chunk_off.release();
-  ctx->d_stream.release();
+  ctx->d_stream.release(); ctx->d_pset.release();
   ctx->d_bin_ids.release(); ctx->d_chist.release(); ctx->d_cbase.release(); ctx->d_bin_off.release(); ctx->d_sorted.release();
   ctx->d_part.release(); ctx->d_labels.release(); ctx->d_fits.release(); ctx->d_segs.release(); ctx->d_wq_ctr.release();
   for (int c = 0; c < NUM_CLASSES; ++c) ctx->d_wq_items[c].release();
   ctx->d_out_idx.release(); ctx->d_counts.release();
   ctx->d_centers.release(); ctx->d_normals.release(); ctx->d_xyz.release();
-  ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); }
+  ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
   ctx->h_out_idx.release(); ctx->h_counts.release();
   ctx->h_centers.release(); ctx->h_normals.release();
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
@@ -1096,7 +1179,7 @@ int pwpp_copy_centers(pwpp_ctx* ctx, int f, float* dst) {
   rc = fetch_patches(ctx);
   if (rc) return rc;
   const int k = count_of(ctx, 1, f);
-  if (k > 0) std::memcpy(dst, ctx->h_centers.p + (size_t) f * ctx->g.nbins * 3, (size_t) k * 3 * sizeof(float));
+  if (k > 0) std::memcpy(dst, ctx->h_centers.p + (size_t) f * ctx->gs.nbs * 3, (size_t) k * 3 * sizeof(float));
   return PWPP_OK;
 }
 int pwpp_copy_normals(pwpp_ctx* ctx, int f, float* dst) {
@@ -1105,7 +1188,7 @@ int pwpp_copy_normals(pwpp_ctx* ctx, int f, float* dst) {
   rc = fetch_patches(ctx);
   if (rc) return rc;
   const int k = count_of(ctx, 1, f);
-  if (k > 0) std::memcpy(dst, ctx->h_normals.p + (size_t) f * ctx->g.nbins * 3, (size_t) k * 3 * sizeof(float));
+  if (k > 0) std::memcpy(dst, ctx->h_normals.p + (size_t) f * ctx->gs.nbs * 3, (size_t) k * 3 * sizeof(float));
   return PWPP_OK;
 }
 
@@ -1150,7 +1233,7 @@ int pwpp_copy_history(pwpp_ctx* ctx, int f, int ring, int which, double* dst) {
   int rc = pwpp_get_state(ctx, f, &s);
   if (rc) return rc;
   const int n = which ? s.n_flatness[ring] : s.n_elevation[ring];
-  if (n > 0) CU_TRY(cudaMemcpy(dst, ctx->d_hist.p + (((size_t) f * 2 + which) * 4 + ring) * ctx->hcap, (size_t) n * sizeof(double), cudaMemcpyDeviceToHost));
+  if (n > 0) CU_TRY(cudaMemcpy(dst, ctx->d_hist.p + (((size_t) f * 2 + which) * 4 + ring) * ctx->hist_stride, (size_t) n * sizeof(double), cudaMemcpyDeviceToHost));
   return PWPP_OK;
 }
 
@@ -1158,9 +1241,13 @@ namespace {
 struct StateBlobHeader { uint32_t magic, version; int32_t hcap, state_bytes; };
 constexpr uint32_t STATE_BLOB_MAGIC = 0x50575354u;  // "PWST"
 }  // namespace
-size_t pwpp_state_blob_size(const pwpp_ctx* ctx) {
-  return ctx ? sizeof(StateBlobHeader) + sizeof(StreamState) + (size_t) 2 * 4 * ctx->hcap * sizeof(double) : 0;
+// a stream's blob: header, state, then its eight history rows of its own set's capacity (the layout of a one-set context)
+static size_t blob_size_of_cap(int hcap) { return sizeof(StateBlobHeader) + sizeof(StreamState) + (size_t) 2 * 4 * hcap * sizeof(double); }
+size_t pwpp_stream_state_blob_size(const pwpp_ctx* ctx, int s) {
+  if (!ctx || s < 0 || s >= ctx->num_streams) return 0;
+  return blob_size_of_cap(ctx->set_hcap[ctx->stream_set[s]]);
 }
+size_t pwpp_state_blob_size(const pwpp_ctx* ctx) { return ctx ? blob_size_of_cap(ctx->hist_stride) : 0; }
 int pwpp_export_state(pwpp_ctx* ctx, int f, void* blob) {
   if (!ctx || !blob || f < 0 || f >= ctx->num_streams) return fail(PWPP_ERR_INVALID_ARG, "bad argument");
   int rc = bind_device(ctx);
@@ -1168,20 +1255,22 @@ int pwpp_export_state(pwpp_ctx* ctx, int f, void* blob) {
   if (ctx->last_stream) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
   CU_TRY(cudaStreamSynchronize(ctx->stream));
   char* b = static_cast<char*>(blob);
-  const StateBlobHeader h{STATE_BLOB_MAGIC, (uint32_t) PWPP_ABI_VERSION, ctx->hcap, (int32_t) sizeof(StreamState)};
+  const int hcap = ctx->set_hcap[ctx->stream_set[f]];
+  const StateBlobHeader h{STATE_BLOB_MAGIC, (uint32_t) PWPP_ABI_VERSION, hcap, (int32_t) sizeof(StreamState)};
   std::memcpy(b, &h, sizeof h);
   CU_TRY(cudaMemcpy(b + sizeof h, ctx->d_states.p + f, sizeof(StreamState), cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(b + sizeof h + sizeof(StreamState), ctx->d_hist.p + (size_t) f * 2 * 4 * ctx->hcap, (size_t) 2 * 4 * ctx->hcap * sizeof(double),
-                    cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemcpy2D(b + sizeof h + sizeof(StreamState), (size_t) hcap * sizeof(double), ctx->d_hist.p + (size_t) f * 2 * 4 * ctx->hist_stride,
+                      (size_t) ctx->hist_stride * sizeof(double), (size_t) hcap * sizeof(double), 2 * 4, cudaMemcpyDeviceToHost));
   return PWPP_OK;
 }
 int pwpp_import_state(pwpp_ctx* ctx, int f, const void* blob, size_t bytes) {
   if (!ctx || !blob || f < 0 || f >= ctx->num_streams) return fail(PWPP_ERR_INVALID_ARG, "bad argument");
-  if (bytes != pwpp_state_blob_size(ctx)) return fail(PWPP_ERR_INVALID_ARG, "state blob has the wrong size for this context (different storage parameters?)");
+  if (bytes != pwpp_stream_state_blob_size(ctx, f)) return fail(PWPP_ERR_INVALID_ARG, "state blob has the wrong size for this context (different storage parameters?)");
+  const int hcap = ctx->set_hcap[ctx->stream_set[f]];
   const char* b = static_cast<const char*>(blob);
   StateBlobHeader h;
   std::memcpy(&h, b, sizeof h);
-  if (h.magic != STATE_BLOB_MAGIC || h.version != (uint32_t) PWPP_ABI_VERSION || h.hcap != ctx->hcap || h.state_bytes != (int32_t) sizeof(StreamState))
+  if (h.magic != STATE_BLOB_MAGIC || h.version != (uint32_t) PWPP_ABI_VERSION || h.hcap != hcap || h.state_bytes != (int32_t) sizeof(StreamState))
     return fail(PWPP_ERR_INVALID_ARG, "not a state blob of this library version / parameter set");
   int rc = bind_device(ctx);
   if (rc) return rc;
@@ -1189,8 +1278,8 @@ int pwpp_import_state(pwpp_ctx* ctx, int f, const void* blob, size_t bytes) {
   if (ctx->last_stream) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
   CU_TRY(cudaStreamSynchronize(ctx->stream));
   CU_TRY(cudaMemcpy(ctx->d_states.p + f, b + sizeof h, sizeof(StreamState), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(ctx->d_hist.p + (size_t) f * 2 * 4 * ctx->hcap, b + sizeof h + sizeof(StreamState), (size_t) 2 * 4 * ctx->hcap * sizeof(double),
-                    cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy2D(ctx->d_hist.p + (size_t) f * 2 * 4 * ctx->hist_stride, (size_t) ctx->hist_stride * sizeof(double), b + sizeof h + sizeof(StreamState),
+                      (size_t) hcap * sizeof(double), (size_t) hcap * sizeof(double), 2 * 4, cudaMemcpyHostToDevice));
   return PWPP_OK;
 }
 
@@ -1260,7 +1349,8 @@ int pwpp_copy_bin_results(pwpp_ctx* ctx, int f, pwpp_bin_result* dst) {
   rc = bind_device(ctx);
   if (rc) return rc;
   CU_TRY(cudaStreamSynchronize(ctx->last_stream));
-  CU_TRY(cudaMemcpy(dst, ctx->d_fits.p + (size_t) f * ctx->g.nbins, (size_t) ctx->g.nbins * sizeof(BinFit), cudaMemcpyDeviceToHost));
+  const int nb = ctx->gs.g[ctx->frame_set[f]].nbins;   // the records of the frame's set
+  CU_TRY(cudaMemcpy(dst, ctx->d_fits.p + (size_t) f * ctx->gs.nbs, (size_t) nb * sizeof(BinFit), cudaMemcpyDeviceToHost));
   return PWPP_OK;
 }
 int pwpp_copy_bin_ids(pwpp_ctx* ctx, int f, uint16_t* dst) {

@@ -25,6 +25,16 @@ inline const int* simt_identity_streams() {
   return v;
 }
 inline const int* g_simt_streams = simt_identity_streams();
+// the parameter-set table of a FrameTable whose initializer names none: every frame on set 0 (a one-set context), unless a
+// harness points it at another table for the duration of a call
+inline const int* simt_zero_sets() {
+  static int v[65536] = {};
+  return v;
+}
+inline const int* g_simt_sets = simt_zero_sets();
+#ifndef __grid_constant__
+#define __grid_constant__
+#endif
 #endif
 
 struct FrameTable {            // per call, device arrays indexed by frame
@@ -33,10 +43,39 @@ struct FrameTable {            // per call, device arrays indexed by frame
   // [F] stream of each frame: index of its StreamState and of its history rows
 #if defined(PWPP_SIMT_EMU)
   const int* stream = g_simt_streams;
+  const int* pset = g_simt_sets;
 #else
   const int* stream;
+  const int* pset;             // [F] parameter set of each frame (the set of its stream): index into GeometrySets / AlgoParamSets
 #endif
 };
+
+// The parameter sets of a context (pwpp_create_sets), passed BY VALUE to every kernel that reads them: the records sit in the
+// kernel's parameter bank, and a kernel reads its frame's record through a reference into it (`__grid_constant__`: no local
+// copy), one indexed constant load per field. Not a __constant__ symbol (contexts on one device would share it), not a global
+// table (the fit kernels have no registers to spare for the extra pointer and loads). A one-set context fills set 0 only; the
+// converting constructors make a single Geometry / AlgoParams the set table of a one-set launch.
+constexpr int MAX_PARAM_SETS = 8;   // PWPP_MAX_PARAM_SETS
+struct GeometrySets {
+  Geometry g[MAX_PARAM_SETS];
+  int nbs;                     // stride of the per-frame bin arrays (patch records, centers, normals): the largest nbins of the sets
+  GeometrySets() = default;
+  __host__ __device__ GeometrySets(const Geometry& g0) : g{g0}, nbs(g0.nbins) {}
+};
+struct AlgoParamSets {
+  AlgoParams a[MAX_PARAM_SETS];
+  AlgoParamSets() = default;
+  __host__ __device__ AlgoParamSets(const AlgoParams& a0) : a{a0} {}
+};
+// both tables plus the other arguments of the kernel with the longest list (k_front_cluster: < 256 bytes) stay inside the
+// classic 4 KB kernel-parameter limit
+static_assert(sizeof(GeometrySets) + sizeof(AlgoParamSets) + 256 <= 4096, "parameter-set tables exceed the kernel parameter space");
+// history row capacity of a set (DESIGN.md section 3, deviation 1): the newest hcap samples of a ring are kept
+__host__ __device__ inline int history_cap(const Geometry& g, const AlgoParams& ap) {
+  int ms = 0;
+  for (int k = 0; k < 4; ++k) ms = g.num_sectors[k] > ms ? g.num_sectors[k] : ms;
+  return (ap.max_elevation_storage > ap.max_flatness_storage ? ap.max_elevation_storage : ap.max_flatness_storage) + 4 * ms + 64;
+}
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 // ---- thread-block clusters (k_front_cluster): rank, barrier, distributed shared memory ----

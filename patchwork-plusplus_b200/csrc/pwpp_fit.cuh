@@ -208,7 +208,7 @@ enum FitState { ST_RVPF = 0, ST_SEED = 1, ST_GPF = 2, ST_FINAL = 3, ST_DONE = 4 
 // Point j of a patch lives in lane (j % G) of the group at register slot (j / G).
 template <int G, int K, int CLS, int MINB>
 __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states,
-                                                                 Geometry g, AlgoParams ap, int nbp, const int* __restrict__ bin_off, WorkQueues wq,
+                                                                 const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps, int nbp, const int* __restrict__ bin_off, WorkQueues wq,
                                                                  int* __restrict__ part, BinFit* __restrict__ fits) {
   static_assert(G == 8 || G == 16 || G == 32, "group is a warp, half a warp or a quarter warp");
   constexpr int NGW = 32 / G;                  // patches per warp
@@ -238,6 +238,9 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
       P = sorted + start;
       out = part + start;
     }
+    const int set = ft.pset[f];                  // the parameter set of this group's frame
+    const Geometry& g = gs.g[set];
+    const AlgoParams& ap = aps.a[set];
     // ---- load the patches of this warp into registers ----
     float px[K], py[K], pz[K];
     unsigned vmask = 0;                        // bit k: slot k holds a point
@@ -408,7 +411,7 @@ __global__ void __launch_bounds__(FIT_THREADS, MINB) k_fit_resident(const float4
         ng_run += __popc(bn);
       }
       if (have && gl == 0) {
-        BinFit& r = fits[(size_t) f * g.nbins + bin];
+        BinFit& r = fits[(size_t) f * gs.nbs + bin];
         r.n = n; r.n_ground = n_ground; r.fitted = 1;
         r.verdict = have_plane ? 0 : PW_FIT_NO_PLANE;
 #pragma unroll
@@ -444,7 +447,7 @@ __device__ __forceinline__ int dist_filter(const PlaneF& pf, float th, float x, 
 // budget of 4 CTAs per SM with far fewer spills.
 template <int CAP, int CLS, int MINB, int NW, bool FUSE = false, bool PLS = false>
 __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states,
-                                                                                Geometry g, AlgoParams ap, int nbp, const int* __restrict__ bin_off, WorkQueues wq,
+                                                                                const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps, int nbp, const int* __restrict__ bin_off, WorkQueues wq,
                                                                                 int* __restrict__ part, BinFit* __restrict__ fits) {
   constexpr int NT = NW * 32;                // NW warps per patch (8 or 16)
   static_assert(NW == 8 || NW == 16, "warp 0 keeps NW minima per lane and splits a patch into NW contiguous chunks");
@@ -469,7 +472,6 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
   __shared__ int4 s_item;
   __shared__ Plane s_plane;
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const float thf = (float) ap.th_dist;
   const int count = wq.count[CLS];
   const int4 no_item = make_int4(-1, 0, 0, 0);
 
@@ -488,6 +490,10 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
     int next_raw = 0;
     if (tid == LOOK_TID) next_raw = atomicAdd(&wq.head[CLS], 1);
     const int f = cur.x >> 12, bin = cur.x & 0xfff, n = cur.y;
+    const int set = ft.pset[f];                  // the frame's parameter set
+    const Geometry& g = gs.g[set];
+    const AlgoParams& ap = aps.a[set];
+    const float thf = (float) ap.th_dist;
     const long long start = work_item_start(cur);
     const float4* P = sorted + start;
     int* out = part + start;
@@ -892,7 +898,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         }
       }
       if (tid == 0) {
-        BinFit& r = fits[(size_t) f * g.nbins + bin];
+        BinFit& r = fits[(size_t) f * gs.nbs + bin];
         r.n = n; r.n_ground = n_ground; r.fitted = 1;
         r.verdict = have_plane ? 0 : PW_FIT_NO_PLANE;
 #pragma unroll
@@ -1121,7 +1127,7 @@ __device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool an
 // test and by the solve. That is what lets the kernel run at 3 CTAs per SM (85 registers) without spilling.
 template <bool STAGE, int CLS_HI, int CLS_LO, int U, int MINB, bool FUSE = false, bool PLS = false>
 __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states,
-                                                                             Geometry g, AlgoParams ap, int nbp, const int* __restrict__ bin_off, WorkQueues wq,
+                                                                             const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps, int nbp, const int* __restrict__ bin_off, WorkQueues wq,
                                                                              int* __restrict__ part, BinFit* __restrict__ fits) {
   constexpr int CAP = STAGE ? CLS_M_MAX : (CLS_HI == 2 ? CLS_L1_MAX : WARP_CAP);
   __shared__ unsigned s_alive[FITW_WARPS][CAP / 32];
@@ -1138,7 +1144,6 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
   float* sel_buf = s_sel[warp];
   int cls = CLS_HI;          // queues being drained, longest patches first
   const int cls_last = CLS_LO;
-  const float thf = (float) ap.th_dist;
   int cnt = wq.count[cls];
   const int4 no_item = make_int4(-1, 0, 0, 0);
   int4 cur = no_item;
@@ -1165,6 +1170,10 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
     int4 nxt = no_item;
     bool looked_ahead = false;
     const int f = cur.x >> 12, bin = cur.x & 0xfff, n = cur.y;
+    const int set = ft.pset[f];                  // the frame's parameter set
+    const Geometry& g = gs.g[set];
+    const AlgoParams& ap = aps.a[set];
+    const float thf = (float) ap.th_dist;
     const long long start = work_item_start(cur);
     const float4* G = sorted + start;           // the patch in global memory
     int* out = part + start;
@@ -1406,7 +1415,7 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
       }
     }
     if (lane == 0) {
-      BinFit& r = fits[(size_t) f * g.nbins + bin];
+      BinFit& r = fits[(size_t) f * gs.nbs + bin];
       r.n = n; r.n_ground = n_ground; r.fitted = 1;
       r.verdict = have_plane ? 0 : PW_FIT_NO_PLANE;
 #pragma unroll

@@ -26,8 +26,8 @@ constexpr int BIG_CCAP = 512;   // candidate buffer of the LPR selection (16 key
 constexpr int BIG_U = 4;        // loads in flight per thread (on dense frames 2 in flight was slower, 8 no faster)
 
 template <int NW, int MINB, bool FUSE>
-__global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states, Geometry g,
-                                                            AlgoParams ap, int nbp, const int* __restrict__ bin_off, WorkQueues wq, int* __restrict__ part,
+__global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states, const __grid_constant__ GeometrySets gs,
+                                                            const __grid_constant__ AlgoParamSets aps, int nbp, const int* __restrict__ bin_off, WorkQueues wq, int* __restrict__ part,
                                                             BinFit* __restrict__ fits) {
   constexpr int NT = NW * 32;
   constexpr int CLS = NUM_CLASSES - 1;
@@ -47,8 +47,6 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
   __shared__ int4 s_item;
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const unsigned lt = lanemask_lt();
-  const float thf = (float) ap.th_dist;
-  const bool fuse_ok = FUSE && (ap.th_seeds <= ap.th_seeds_v);
 
   for (;;) {
     if (tid == 0) {
@@ -59,6 +57,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
     const int4 cur = s_item;
     if (cur.x < 0) return;
     const int f = cur.x >> 12, bin = cur.x & 0xfff, n = cur.y;
+    const int set = ft.pset[f];                  // the frame's parameter set
+    const Geometry& g = gs.g[set];
+    const AlgoParams& ap = aps.a[set];
+    const float thf = (float) ap.th_dist;
+    const bool fuse_ok = FUSE && (ap.th_seeds <= ap.th_seeds_v);
     const long long start = work_item_start(cur);
     const float4* P = sorted + start;
     int* out = part + start;
@@ -399,7 +402,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_big(const float4* __restr
       for (int i = tid; i < n; i += NT) { out[i] = __float_as_int(P[i].w); if (wq.labels) wq.labels[start + i] = PW_LABEL_REJECT; }
     }
     if (tid == 0) {
-      BinFit& r = fits[(size_t) f * g.nbins + bin];
+      BinFit& r = fits[(size_t) f * gs.nbs + bin];
       r.n = n; r.n_ground = n_ground; r.fitted = 1;
       r.verdict = have_plane ? 0 : PW_FIT_NO_PLANE;
 #pragma unroll

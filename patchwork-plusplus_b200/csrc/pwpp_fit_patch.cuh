@@ -93,8 +93,8 @@ __device__ __noinline__ bool exact_below(float x, float y, float z, const double
 }
 
 template <int NW, int MINB, int CLS>
-__global__ void __launch_bounds__(NW * 32, MINB) k_fit_patch(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states, Geometry g,
-                                                              AlgoParams ap, int nbp, const int* __restrict__ bin_off, WorkQueues wq, int* __restrict__ part,
+__global__ void __launch_bounds__(NW * 32, MINB) k_fit_patch(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states, const __grid_constant__ GeometrySets gs,
+                                                              const __grid_constant__ AlgoParamSets aps, int nbp, const int* __restrict__ bin_off, WorkQueues wq, int* __restrict__ part,
                                                               BinFit* __restrict__ fits) {
   constexpr int NT = NW * 32;
   constexpr int M_TOP = 32 / NW;   // smallest lane minima each warp contributes to the bound
@@ -114,9 +114,6 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_patch(const float4* __res
   PW_DYN_SHARED(float4, s_stage);   // [NW][FP_STG] compaction buffers of the accumulation
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const unsigned lt = lanemask_lt();
-  const float thf = (float) ap.th_dist;
-  const bool fuse_ok = ap.th_seeds <= ap.th_seeds_v;
-  const int K = ap.num_lpr;
   const int count = wq.count[CLS];
   PW_EV_DECL;
 
@@ -139,6 +136,12 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_patch(const float4* __res
       if (t < count) nxt = wq.items[CLS][t];
     }
     const int f = cur.x >> 12, bin = cur.x & 0xfff, n = cur.y;
+    const int set = ft.pset[f];                  // the frame's parameter set
+    const Geometry& g = gs.g[set];
+    const AlgoParams& ap = aps.a[set];
+    const float thf = (float) ap.th_dist;
+    const bool fuse_ok = ap.th_seeds <= ap.th_seeds_v;
+    const int K = ap.num_lpr;
     const long long start = work_item_start(cur);
     const float4* P = sorted + start;
     int* out = part + start;
@@ -589,7 +592,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_patch(const float4* __res
         }
       }
       if (tid == 0) {
-        BinFit& r = fits[(size_t) f * g.nbins + bin];
+        BinFit& r = fits[(size_t) f * gs.nbs + bin];
         r.n = n; r.n_ground = n_ground; r.fitted = 1;
         r.verdict = have_plane ? 0 : PW_FIT_NO_PLANE;
 #pragma unroll

@@ -49,8 +49,9 @@ __global__ void
 #if !defined(PWPP_SIMT_EMU)
 __cluster_dims__(FC_CS, 1, 1)
 #endif
-__launch_bounds__(NT, 1024 / NT) k_front_cluster(const float4* __restrict__ pts, FrameTable ft, const StreamState* __restrict__ states, Geometry g, AlgoParams ap,
-                                                  int has_intensity, int nbp, int nbins, unsigned short* __restrict__ bin_ids, int* __restrict__ bin_off, WorkQueues wq,
+__launch_bounds__(NT, 1024 / NT) k_front_cluster(const float4* __restrict__ pts, FrameTable ft, const StreamState* __restrict__ states,
+                                                  const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps,
+                                                  int has_intensity, int nbp, int nbs, unsigned short* __restrict__ bin_ids, int* __restrict__ bin_off, WorkQueues wq,
                                                   BinFit* __restrict__ fits, float4* __restrict__ sorted) {
   constexpr int FC_THREADS = NT, FC_WARPS = NT / 32;   // (shadow the namespace-scope defaults)
   PW_DYN_SHARED(unsigned char, s_raw);
@@ -70,6 +71,10 @@ __launch_bounds__(NT, 1024 / NT) k_front_cluster(const float4* __restrict__ pts,
   const int i0 = (int) ((long long) nrows * gw / (FC_CS * FC_WARPS)) << 5;                        // this warp's points [i0, i1)
   const int i1 = min(n, (int) ((long long) nrows * (gw + 1) / (FC_CS * FC_WARPS)) << 5);
   const float4* fp = pts + p0;
+  const int set = ft.pset[f];                                                                     // the frame's parameter set
+  const Geometry& g = gs.g[set];
+  const AlgoParams& ap = aps.a[set];
+  const int nbins = g.nbins;
   const double sensor_height = states[ft.stream[f]].sensor_height;
   const bool rnr_on = ap.enable_RNR && has_intensity;  // S:161, S:379-382
   unsigned* my = s_wb + (size_t) w * nbp;
@@ -185,7 +190,7 @@ __launch_bounds__(NT, 1024 / NT) k_front_cluster(const float4* __restrict__ pts,
       const int m = s_scan[b + 1] - s_scan[b];
       if (m >= ap.num_min_pts && m > 0) atomicAdd(&s_cnt[cls_of(m)], 1);
       else {
-        BinFit& r = fits[(size_t) f * nbins + b];
+        BinFit& r = fits[(size_t) f * nbs + b];
         r.n = m; r.n_ground = 0; r.d = 0.0;
         for (int k = 0; k < 3; ++k) { r.mean[k] = 0.0; r.normal[k] = 0.0; r.sv[k] = 0.0; }
         r.fitted = (m >= ap.num_min_pts) ? 1 : 0;   // an EMPTY patch with num_min_pts <= 0 is "fitted" with the previous patch's plane (S:49)

@@ -36,7 +36,8 @@ namespace pwpp {
 // flight while the current one is binned (PWPP_HIST_PIPE, A/B switch)
 template <bool FAST, int PIPE>
 __global__ void __launch_bounds__(CHUNK_THREADS, 4) k_bin_hist(const float4* __restrict__ pts, FrameTable ft, const StreamState* __restrict__ states,
-                                                             Geometry g, AlgoParams ap, int has_intensity, int nbp,
+                                                             const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps,
+                                                             int has_intensity, int nbp,
                                                              unsigned short* __restrict__ bin_ids, unsigned short* __restrict__ chist) {
   PW_DYN_SHARED(unsigned int, s_hist);  // [nbp]
   const int f = blockIdx.y;
@@ -46,6 +47,9 @@ __global__ void __launch_bounds__(CHUNK_THREADS, 4) k_bin_hist(const float4* __r
   if ((int) blockIdx.x >= nchunks) return;
   for (int b = threadIdx.x; b < nbp; b += CHUNK_THREADS) s_hist[b] = 0;
   __syncthreads();
+  const int set = ft.pset[f];   // the frame's parameter set
+  const Geometry& g = gs.g[set];
+  const AlgoParams& ap = aps.a[set];
   const double sensor_height = states[ft.stream[f]].sensor_height;
   const bool rnr_on = ap.enable_RNR && has_intensity;  // S:161, S:379-382
   const int warp = threadIdx.x >> 5, lane = lane_id();
@@ -98,12 +102,16 @@ __global__ void __launch_bounds__(CHUNK_THREADS, 4) k_bin_hist(const float4* __r
 // cbase[chunk][b] = position where chunk's first point of bin b goes.
 // Also sorts the frame's patches into the work queues of the fit kernels by size (S:191: patches below
 // num_min_pts are not fitted) and initialises the BinFit records of the patches that will not be fitted.
+// nbs is the stride of the patch records; the frame's bin count and num_min_pts are those of its parameter set.
 template <int L2MAX, int MMAX = CLS_M_MAX>
-__global__ void k_bin_scan(FrameTable ft, int nbp, int nbins, int num_min_pts, const unsigned short* __restrict__ chist, unsigned int* __restrict__ cbase,
-                           int* __restrict__ bin_off, WorkQueues wq, BinFit* __restrict__ fits) {
+__global__ void k_bin_scan(FrameTable ft, int nbp, int nbs, const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps,
+                           const unsigned short* __restrict__ chist, unsigned int* __restrict__ cbase, int* __restrict__ bin_off, WorkQueues wq,
+                           BinFit* __restrict__ fits) {
   PW_DYN_SHARED(int, s_scan);  // [nbp + 1]
   __shared__ int s_cls_cnt[NUM_CLASSES], s_cls_base[NUM_CLASSES], s_cls_pos[NUM_CLASSES];
   const int f = blockIdx.x;
+  const int set = ft.pset[f];
+  const int nbins = gs.g[set].nbins, num_min_pts = aps.a[set].num_min_pts;
   const int c0 = ft.chunk_off[f], c1 = ft.chunk_off[f + 1];
   if (threadIdx.x < NUM_CLASSES) { s_cls_cnt[threadIdx.x] = 0; s_cls_pos[threadIdx.x] = 0; }
   for (int b = threadIdx.x; b < nbp; b += blockDim.x) {
@@ -143,7 +151,7 @@ __global__ void k_bin_scan(FrameTable ft, int nbp, int nbins, int num_min_pts, c
     const int n = s_scan[b + 1] - s_scan[b];
     if (n >= num_min_pts && n > 0) atomicAdd(&s_cls_cnt[cls_of(n)], 1);
     else {
-      BinFit& r = fits[(size_t) f * nbins + b];
+      BinFit& r = fits[(size_t) f * nbs + b];
       r.n = n; r.n_ground = 0; r.d = 0.0;
       for (int k = 0; k < 3; ++k) { r.mean[k] = 0.0; r.normal[k] = 0.0; r.sv[k] = 0.0; }
       // an EMPTY patch with num_min_pts <= 0 is "fitted" by the reference with the previous patch's plane (S:49)
@@ -162,6 +170,19 @@ __global__ void k_bin_scan(FrameTable ft, int nbp, int nbins, int num_min_pts, c
     }
   }
 }
+
+#if defined(PWPP_SIMT_EMU)
+// tests/simt: the one-set launch with the frame's bin count and num_min_pts as scalars (what the CPU twin passes)
+template <int L2MAX, int MMAX = CLS_M_MAX>
+inline void k_bin_scan(FrameTable ft, int nbp, int nbins, int num_min_pts, const unsigned short* chist, unsigned int* cbase, int* bin_off, WorkQueues wq,
+                       BinFit* fits) {
+  Geometry g{};
+  g.nbins = nbins;
+  AlgoParams ap{};
+  ap.num_min_pts = num_min_pts;
+  k_bin_scan<L2MAX, MMAX>(ft, nbp, nbins, GeometrySets(g), AlgoParamSets(ap), chist, cbase, bin_off, wq, fits);
+}
+#endif
 
 // ---------------------------------------------------------------------------------------------------
 // k_scatter: same decomposition as k_bin_hist. Stable: a point's position inside its bin is its rank
@@ -276,8 +297,10 @@ constexpr int GLE_CH = 128;   // samples of each history row staged per step of 
 __host__ __device__ inline size_t gle_smem_bytes(int max_sectors) { return (size_t) 6 * max_sectors * sizeof(double) + (size_t) 2 * max_sectors * sizeof(int) + (size_t) 8 * GLE_CH * sizeof(double); }
 #define PW_SEG_TO_NG(x) (-3 - (x))   /* "ground part goes to the non-ground list at offset x" until the final shift */
 
-__global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restrict__ states, double* __restrict__ hist, int hcap, Geometry g, AlgoParams ap,
-                                            int nbp, int max_sectors, const int* __restrict__ bin_off, BinFit* __restrict__ fits, BinSeg* __restrict__ segs,
+// hist_stride is the row stride of the histories (the largest history_cap of the sets); the logical capacity of a stream's rows
+// is its own set's history_cap, exactly as in a context created with that set alone. max_sectors sizes the shared memory.
+__global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restrict__ states, double* __restrict__ hist, int hist_stride,
+                                            const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps, int nbp, int max_sectors, const int* __restrict__ bin_off, BinFit* __restrict__ fits, BinSeg* __restrict__ segs,
                                             int* __restrict__ num_ground, int* __restrict__ num_patches, float* __restrict__ centers, float* __restrict__ normals,
                                             int* __restrict__ num_dropped) {
   PW_DYN_SHARED(double, s_gle);
@@ -291,15 +314,19 @@ __global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restri
   const int lane = lane_id();
   const unsigned lt = lanemask_lt();
   const int sid = ft.stream[f];                       // frame f of the call advances stream sid
+  const int set = ft.pset[f];                         // with the parameters of its set
+  const Geometry& g = gs.g[set];
+  const AlgoParams& ap = aps.a[set];
   StreamState& st = states[sid];
   const int nb = g.nbins, nb_all = nb + PW_NUM_PSEUDO;
+  const int hcap = history_cap(g, ap);
   const int* bo = bin_off + (size_t) f * (nbp + 1);
-  BinFit* fit = fits + (size_t) f * nb;
-  BinSeg* seg = segs + (size_t) f * nb_all;
-  float* cen = centers + (size_t) f * nb * 3;
-  float* nor = normals + (size_t) f * nb * 3;
-  double* h_elev = hist + ((size_t) sid * 2 + 0) * 4 * hcap;
-  double* h_flat = hist + ((size_t) sid * 2 + 1) * 4 * hcap;
+  BinFit* fit = fits + (size_t) f * gs.nbs;
+  BinSeg* seg = segs + (size_t) f * (gs.nbs + PW_NUM_PSEUDO);
+  float* cen = centers + (size_t) f * gs.nbs * 3;
+  float* nor = normals + (size_t) f * gs.nbs * 3;
+  double* h_elev = hist + ((size_t) sid * 2 + 0) * 4 * hist_stride;
+  double* h_flat = hist + ((size_t) sid * 2 + 1) * 4 * hist_stride;
 
 #if !defined(PWPP_SIMT_EMU)
   // The ring loop below is a chain of ~20 dependent round trips to this frame's patch records (104 B each, written by the fit
@@ -401,8 +428,8 @@ __global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restri
         const unsigned pm = __ballot_sync(0xffffffffu, push);
         if (pm) {
           const int cnt = __popc(pm);
-          double* he = h_elev + ci * hcap;
-          double* hf = h_flat + ci * hcap;
+          double* he = h_elev + ci * hist_stride;
+          double* hf = h_flat + ci * hist_stride;
           int ne = n_e[0], nf = n_f[0];
 #pragma unroll
           for (int i = 1; i < 4; ++i) if (ci == i) { ne = n_e[i]; nf = n_f[i]; }
@@ -533,7 +560,7 @@ __global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restri
 #pragma unroll
         for (int r = 0; r < 8; ++r) {
           const int nr = __shfl_sync(0xffffffffu, my_n, r);
-          const double* src = (r < 4 ? h_elev + r * hcap : h_flat + (r - 4) * hcap) + c0;
+          const double* src = (r < 4 ? h_elev + r * hist_stride : h_flat + (r - 4) * hist_stride) + c0;
           const int len = min(GLE_CH, nr - c0);
           for (int i = lane; i < len; i += 32) s_h[r * GLE_CH + i] = src[i];
         }
@@ -575,7 +602,7 @@ __global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restri
       const int exceed = nn - (which ? ap.max_flatness_storage : ap.max_elevation_storage);
       const bool doit = which ? (((flat_upd_mask >> r) & 1u) != 0) : (nn > 0);
       if (doit && exceed > 0) {
-        double* a = (which ? h_flat : h_elev) + r * hcap;
+        double* a = (which ? h_flat : h_elev) + r * hist_stride;
         for (int i0 = 0; i0 < nn - exceed; i0 += 32) {
           const int i = i0 + lane;
           double t = 0.0;
@@ -604,7 +631,7 @@ __global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restri
 constexpr int EMIT_WARPS = 8;
 constexpr int EMIT_TILE = 1024;
 
-__global__ void __launch_bounds__(EMIT_WARPS * 32) k_emit(FrameTable ft, Geometry g, int nbp, const int* __restrict__ bin_off, const BinFit* __restrict__ fits,
+__global__ void __launch_bounds__(EMIT_WARPS * 32) k_emit(FrameTable ft, const __grid_constant__ GeometrySets gs, int nbp, const int* __restrict__ bin_off, const BinFit* __restrict__ fits,
                                                                 const BinSeg* __restrict__ segs, const int* __restrict__ part, const float4* __restrict__ sorted,
                                                                 int* __restrict__ out_idx) {
   const int f = blockIdx.y;
@@ -614,7 +641,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32) k_emit(FrameTable ft, Geometr
   const int w0 = (blockIdx.x * EMIT_WARPS + (threadIdx.x >> 5)) * EMIT_TILE;
   if (w0 >= n) return;
   const int w1 = min(n, w0 + EMIT_TILE);
-  const int nb_all = g.nbins + PW_NUM_PSEUDO;
+  const int nb = gs.g[ft.pset[f]].nbins, nb_all = nb + PW_NUM_PSEUDO;   // the bins of the frame's parameter set
   const int* bo = bin_off + (size_t) f * (nbp + 1);
   // largest b with bo[b] <= w0: the bin that holds position w0 (empty bins share their offset with the next bin)
   int lo = 0, hi = nb_all;
@@ -634,9 +661,9 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32) k_emit(FrameTable ft, Geometr
     const bool need = valid && end > off && off < w1 && end > w0;
     int g_dst = -1, ng_dst = -1, ng = -1;
     if (need) {
-      const BinSeg sg = segs[(size_t) f * nb_all + b];
+      const BinSeg sg = segs[(size_t) f * (gs.nbs + PW_NUM_PSEUDO) + b];
       g_dst = sg.g_dst; ng_dst = sg.ng_dst;
-      if (b < g.nbins) { const BinFit& r = fits[(size_t) f * g.nbins + b]; if (r.fitted) ng = r.n_ground; }
+      if (b < nb) { const BinFit& r = fits[(size_t) f * gs.nbs + b]; if (r.fitted) ng = r.n_ground; }
     }
     for (unsigned m = __ballot_sync(0xffffffffu, need); m; m &= m - 1) {
       const int l = __ffs(m) - 1;

@@ -32,6 +32,10 @@ def load_library():
     lib.pwpp_last_error.argtypes = []; lib.pwpp_last_error.restype = C.c_char_p
     lib.pwpp_abi_version.argtypes = []; lib.pwpp_abi_version.restype = i32
     lib.pwpp_num_bins.argtypes = [vp]; lib.pwpp_num_bins.restype = i32
+    lib.pwpp_create_sets.argtypes = [C.POINTER(PwppParams), i32, vp, i32, i32, i64, C.POINTER(vp)]; lib.pwpp_create_sets.restype = i32
+    lib.pwpp_stream_num_bins.argtypes = [vp, i32]; lib.pwpp_stream_num_bins.restype = i32
+    lib.pwpp_stream_set.argtypes = [vp, i32]; lib.pwpp_stream_set.restype = i32
+    lib.pwpp_stream_state_blob_size.argtypes = [vp, i32]; lib.pwpp_stream_state_blob_size.restype = C.c_size_t
     lib.pwpp_estimate_host.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(i64), i32, i64, i64]; lib.pwpp_estimate_host.restype = i32
     lib.pwpp_estimate_device.argtypes = [vp, i32, vp, C.POINTER(i64), i32, vp]; lib.pwpp_estimate_device.restype = i32
     lib.pwpp_estimate_host_streams.argtypes = [vp, i32, vp, C.POINTER(vp), C.POINTER(i64), i32, i64, i64]
@@ -83,17 +87,35 @@ def _check(rc):
 
 
 class Engine:
-    """One `pwpp_ctx`: `num_streams` independent sensor streams on one CUDA device."""
+    """One `pwpp_ctx`: `num_streams` independent sensor streams on one CUDA device.
 
-    def __init__(self, params: PwppParams = None, device: int = 0, num_streams: int = 1, max_points_per_frame: int = 0):
+    `params` is one PwppParams (every stream runs with it), or a list of up to 8 parameter sets together with `stream_set`,
+    the set of every stream (pwpp_create_sets): stream s then runs with params[stream_set[s]] for its whole life."""
+
+    def __init__(self, params=None, device: int = 0, num_streams: int = 1, max_points_per_frame: int = 0, stream_set=None):
         self.lib = load_library()
-        self.params = params if params is not None else default_params()
         h = C.c_void_p()
-        _check(self.lib.pwpp_create(C.byref(self.params), device, num_streams, max_points_per_frame, C.byref(h)))
+        if isinstance(params, (list, tuple)):
+            if stream_set is None:
+                raise PwppError("a list of parameter sets needs stream_set, the set of every stream")
+            sets = (PwppParams * max(len(params), 1))(*params)
+            ids = np.ascontiguousarray(stream_set, dtype=np.int32)
+            if ids.shape != (num_streams,):
+                raise PwppError(f"stream_set must name one set per stream ({num_streams}), got shape {ids.shape}")
+            _check(self.lib.pwpp_create_sets(sets, len(params), ids.ctypes.data, device, num_streams, max_points_per_frame, C.byref(h)))
+            self.params = list(params)
+            self.stream_set = ids.tolist()
+        else:
+            if stream_set is not None and any(int(k) != 0 for k in stream_set):
+                raise PwppError("stream_set names sets other than 0, but only one parameter set was given")
+            self.params = params if params is not None else default_params()
+            _check(self.lib.pwpp_create(C.byref(self.params), device, num_streams, max_points_per_frame, C.byref(h)))
+            self.stream_set = [0] * num_streams
         self._h = h
         self.num_streams = num_streams
-        self.nbins = self.lib.pwpp_num_bins(h)
+        self.nbins = self.lib.pwpp_num_bins(h)   # with several sets: the largest bin count of the sets
         self._n = []
+        self._streams = []   # stream of every frame of the last call
 
     def close(self):
         if getattr(self, "_h", None):
@@ -134,12 +156,14 @@ class Engine:
             ids = self._stream_table(streams, nf)
             _check(self.lib.pwpp_estimate_host_streams(self._h, nf, ids.ctypes.data, ptrs, ns, cols, cols, 1))
         self._n = [f.shape[0] for f in frames]
+        self._streams = list(range(nf)) if streams is None else [int(s) for s in streams]
 
     def estimate_host_strided(self, ptrs, ns, cols, row_stride, col_stride):
         nf = len(ptrs)
         p = (C.c_void_p * nf)(*ptrs)
         n = (C.c_int64 * nf)(*ns)
         self._n = list(ns)
+        self._streams = list(range(nf))
         _check(self.lib.pwpp_estimate_host(self._h, nf, p, n, cols, row_stride, col_stride))
 
     def estimate_device(self, d_ptr: int, offsets, has_intensity: bool = True, stream: int = 0, streams=None):
@@ -154,6 +178,7 @@ class Engine:
             _check(self.lib.pwpp_estimate_device_streams(self._h, nf, ids.ctypes.data, C.c_void_p(d_ptr), offs, 1 if has_intensity else 0,
                                                          C.c_void_p(stream)))
         self._n = np.diff(offsets).tolist()
+        self._streams = list(range(nf)) if streams is None else [int(s) for s in streams]
 
     def synchronize(self):
         _check(self.lib.pwpp_synchronize(self._h))
@@ -197,8 +222,17 @@ class Engine:
         _check(self.lib.pwpp_call_times_us(self._h, arr))
         return dict(zip(("h2d", "kernels", "d2h", "device_total"), (float(v) for v in arr)))
 
+    def stream_num_bins(self, s: int) -> int:
+        """Bin count of stream s's parameter set."""
+        n = int(self.lib.pwpp_stream_num_bins(self._h, s))
+        if n < 0:
+            _check(n)
+        return n
+
     def bin_results(self, f=0):
-        arr = (PwppBinResult * self.nbins)()
+        """Patch records of frame f of the last call: the bins of the frame's parameter set."""
+        nb = self.stream_num_bins(self._streams[f]) if 0 <= f < len(self._streams) else self.nbins   # (a bad f: the C-ABI reports it)
+        arr = (PwppBinResult * nb)()
         _check(self.lib.pwpp_copy_bin_results(self._h, f, C.byref(arr)))
         return arr
 
@@ -222,7 +256,7 @@ class Engine:
 
     def export_state(self, f=0) -> bytes:
         """Complete temporal state of stream f as an opaque blob (checkpoint / migration to another ctx or GPU)."""
-        buf = C.create_string_buffer(self.lib.pwpp_state_blob_size(self._h))
+        buf = C.create_string_buffer(self.lib.pwpp_stream_state_blob_size(self._h, f))
         _check(self.lib.pwpp_export_state(self._h, f, buf))
         return buf.raw
 
