@@ -131,6 +131,24 @@ class PatchWorkpp {
     n_ = n;
     ran_ = true;
   }
+  // Sensor records of any PointCloud2 layout (pwpp_estimate_host_records / pwpp_estimate_device_records): n records of
+  // layout.point_step bytes at `data`, unpacked on the GPU. on_device: `data` is device memory, with the stream rules of
+  // estimateGroundDevice. RNR runs when the layout has an intensity field of any datatype.
+  void estimateGroundRecords(const void* data, int64_t n, const pwpp_point_layout& layout, bool on_device = false, void* stream = nullptr) {
+    if (layout.offset[3] < 0 && params_.enable_RNR) std::cout << "RNR requires intensity information !" << std::endl;  // reference src :380
+    const void* frames[1] = {data};
+    const int64_t ns[1] = {n};
+    const int32_t streams[1] = {0};
+    if (on_device) {
+      if (!stream) check(pwpp_device_synchronize(ctx_));
+      check(pwpp_estimate_device_records(ctx_, 1, streams, frames, ns, &layout, stream));
+      if (!stream) check(pwpp_device_synchronize(ctx_));
+    } else {
+      check(pwpp_estimate_host_records(ctx_, 1, streams, frames, ns, &layout));
+    }
+    n_ = n;
+    ran_ = true;
+  }
   // device views of the last call's index lists (int32, valid until the next estimateGround*): {pointer, count}
   std::pair<const int32_t*, int64_t> groundIndicesDevice() {
     const int32_t* idx = nullptr;

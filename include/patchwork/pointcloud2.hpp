@@ -14,6 +14,7 @@
 
 #include <cstring>
 #include <stdexcept>
+#include <string>
 #include <vector>
 
 #include "patchwork/patchworkpp.h"
@@ -50,6 +51,53 @@ inline bool estimateGround(PatchWorkpp& pw, const PointCloud2View& v) {
     for (int c = 0; c < cols; ++c) std::memcpy(&packed[(size_t) i * cols + c], v.data + (size_t) i * v.point_step + offs[c], 4);
   pw.estimateGround(packed.data(), v.num_points, cols, cols, 1);
   return false;
+}
+
+// The description of a sensor_msgs::msg::PointCloud2 as the message carries it: every field's name, offset, datatype
+// (sensor_msgs/PointField codes = PWPP_FIELD_*) and count, plus is_bigendian. A ROS 2 node fills it from the message:
+//   for (auto& f : msg->fields) m.fields.push_back({f.name, f.offset, f.datatype, f.count});
+struct PointField {
+  std::string name;
+  uint32_t offset = 0;
+  uint8_t datatype = 0;
+  uint32_t count = 1;
+};
+struct PointCloud2Message {
+  const uint8_t* data = nullptr;   // msg->data.data()
+  int64_t num_points = 0;          // width * height
+  uint32_t point_step = 0;
+  bool is_bigendian = false;
+  std::vector<PointField> fields;
+};
+
+// The record layout of a message: fields `x`, `y`, `z` and, when present, `intensity`, found by name (the fields the reference
+// node's iterators read, ros/src/Utils.hpp:158-172). Throws std::invalid_argument for a big-endian message, a used field with
+// count != 1 and missing x / y / z; the datatypes and offsets themselves are checked by the engine.
+inline pwpp_point_layout pointLayout(const PointCloud2Message& m) {
+  if (m.is_bigendian) throw std::invalid_argument("PointCloud2Message: big-endian records are not supported");
+  static const char* names[4] = {"x", "y", "z", "intensity"};
+  pwpp_point_layout L;
+  L.point_step = (int32_t) m.point_step;
+  for (int c = 0; c < 4; ++c) {
+    L.offset[c] = -1;
+    L.datatype[c] = 0;
+    for (const PointField& f : m.fields) {
+      if (f.name != names[c]) continue;
+      if (f.count != 1) throw std::invalid_argument(std::string("PointCloud2Message: field ") + names[c] + " has count != 1");
+      L.offset[c] = (int32_t) f.offset;
+      L.datatype[c] = f.datatype;
+      break;
+    }
+    if (c < 3 && L.offset[c] < 0) throw std::invalid_argument(std::string("PointCloud2Message: no field ") + names[c]);
+  }
+  return L;
+}
+
+// estimateGround on a message of any layout (reference GroundSegmentationServer.cpp:74-78): the records go to the GPU as they
+// are and are unpacked there, intensity of any datatype included (RNR then runs, unlike the reference node, :46-47).
+inline void estimateGround(PatchWorkpp& pw, const PointCloud2Message& m) {
+  if (m.num_points < 0 || (m.num_points > 0 && !m.data)) throw std::invalid_argument("PointCloud2Message: bad buffer");
+  pw.estimateGroundRecords(m.data, m.num_points, pointLayout(m));
 }
 
 // Payload of an outgoing x/y/z PointCloud2 (reference Utils.hpp:174-195 EigenMatToPointCloud2 -> FillPointCloud2XYZ):

@@ -192,6 +192,54 @@ int pwpp_estimate_host_streams(pwpp_ctx* ctx, int nframes, const int32_t* stream
 int pwpp_estimate_device_streams(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* d_pts, const int64_t* h_offsets,
                                  int has_intensity, void* cuda_stream);
 
+/* ---- sensor point records of any PointCloud2 layout ------------------------------------------------------------------
+ * A frame may also be handed over as the sensor driver published it: n[f] records of layouts[f].point_step bytes starting at
+ * frames[f] (any alignment, any step: 22, 13 and 17 are as valid as 16), with the byte offset and datatype of the x, y, z and
+ * intensity fields inside a record (sensor_msgs/PointField). One kernel unpacks every frame of a launch range on the GPU into
+ * the ctx's own float4 input buffer; everything after that is the path of pwpp_estimate_host / pwpp_estimate_device.
+ *   - Every frame carries its own layout, so one call may mix sensors of different drivers. Results by call position, state
+ *     by stream id, parameters by the stream's set, layout by the frame. The stream table (required, non-NULL) works exactly
+ *     as for the *_streams entry points: same checks, same error codes, same run splitting.
+ *   - Fields are converted to float by value with round-to-nearest-even (numpy's astype(np.float32)); FLOAT32 passes through
+ *     bit for bit. A FLOAT64 NaN becomes the quiet float NaN with the same sign and the top payload bits. Records are
+ *     little-endian.
+ *   - A frame whose layout has no intensity field (offset[3] < 0) is segmented exactly like an N x 3 frame (RNR skipped,
+ *     S:379-382), even when other frames of the call carry intensity: its points get a NaN intensity, which no RNR test
+ *     accepts, and the call runs with intensity on when any of its frames has it.
+ *   - No byte outside [frames[f], frames[f] + n[f] * point_step) is read.
+ *   - Checked before anything is allocated or launched (the message names the frame and the field); no stream's state
+ *     changes on an error. PWPP_ERR_INVALID_ARG: a NULL streams / frames / n / layouts array, a NULL frame pointer with
+ *     n > 0, n < 0, point_step < 1, an unknown datatype code, a field that does not fit inside point_step.
+ *     PWPP_ERR_UNSUPPORTED: x / y / z not FLOAT32 or FLOAT64, point_step > PWPP_MAX_POINT_STEP.
+ *   - After the call the unpacked points live in the ctx: every getter works as after the other entry points, and the xyz
+ *     getters stay correct after the caller frees or reuses its record buffer.
+ * pwpp_launch_count rises by one unpack launch per pipeline chunk that holds points (host) or per call (device). */
+#define PWPP_FIELD_INT8 1    /* sensor_msgs/PointField datatype codes */
+#define PWPP_FIELD_UINT8 2
+#define PWPP_FIELD_INT16 3
+#define PWPP_FIELD_UINT16 4
+#define PWPP_FIELD_INT32 5
+#define PWPP_FIELD_UINT32 6
+#define PWPP_FIELD_FLOAT32 7
+#define PWPP_FIELD_FLOAT64 8
+#define PWPP_MAX_POINT_STEP 1024
+
+typedef struct pwpp_point_layout {
+  int32_t point_step;   /* bytes from one point to the next (PointCloud2::point_step), 1..PWPP_MAX_POINT_STEP */
+  int32_t offset[4];    /* byte offsets of x, y, z, intensity inside a point; offset[3] < 0: no intensity field */
+  int32_t datatype[4];  /* PWPP_FIELD_*; x, y, z must be FLOAT32 or FLOAT64, intensity any of the eight */
+} pwpp_point_layout;
+
+/* Host-resident records. Every frame's bytes travel as they are (no per-point host loop): a page-locked buffer by DMA
+ * straight from it, a pageable one by one memcpy into page-locked staging and then DMA. The unpack runs on the upload stream
+ * of the pipeline, so pwpp_call_times_us's host->device phase includes it. */
+int pwpp_estimate_host_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames,
+                               const int64_t* n, const pwpp_point_layout* layouts /* [nframes] */);
+/* Device-resident records: unpacked on `cuda_stream` (NULL = the ctx's own stream) with the stream-ordering rules of
+ * pwpp_estimate_device_xyz; the records must stay untouched until the call's work on that stream has run. */
+int pwpp_estimate_device_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* d_frames,
+                                 const int64_t* n, const pwpp_point_layout* layouts /* [nframes] */, void* cuda_stream);
+
 /* cudaDeviceSynchronize() on the ctx's device: what a binding calls before handing device memory produced on an unknown
  * stream to pwpp_estimate_device (and what makes its results visible to every stream afterwards). */
 int pwpp_device_synchronize(pwpp_ctx* ctx);

@@ -76,6 +76,11 @@ def build_examples(force=False):
     if force or _newer(out3, [src3, hdr, os.path.join(REPO, "include", "patchwork", "pointcloud2.hpp"), core]):
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + os.path.join(REPO, "include"), src3, "-o", out3,
                                "-L" + LIB, "-lpwpp_b200", "-Wl,-rpath,$ORIGIN"])
+    src4 = os.path.join(REPO, "tests", "pc2_records_driver.cpp")   # the records path of pointcloud2.hpp against the real engine (GPU test)
+    out4 = os.path.join(LIB, "pc2_records_driver")
+    if force or _newer(out4, [src4, hdr, os.path.join(REPO, "include", "patchwork", "pointcloud2.hpp"), core]):
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + os.path.join(REPO, "include"), src4, "-o", out4,
+                               "-L" + LIB, "-lpwpp_b200", "-Wl,-rpath,$ORIGIN"])
     return out
 
 

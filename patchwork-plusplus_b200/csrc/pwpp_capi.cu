@@ -16,6 +16,7 @@
 
 #include "pwpp.h"
 #include "pwpp_kernels.cuh"
+#include "pwpp_records.cuh"
 #include "pwpp_tuning.h"
 #include "pwpp_host.hpp"
 
@@ -163,12 +164,16 @@ struct pwpp_ctx {
   DevBuf<int> d_counts;           // [3][F]: num_ground, num_patches, num_dropped (F = frames of the call)
   DevBuf<float> d_centers, d_normals;  // [F][nbins][3]
   DevBuf<float> d_xyz;            // gather scratch
+  DevBuf<unsigned char> d_raw;    // pwpp_estimate_host_records: the frames' records as uploaded, unpacked on the device
+  DevBuf<RecordFrame> d_rec;      // [F] record table of a records call
 
   PinBuf<float4> h_in;
   PinBuf<long long> h_pt_off_buf[2];      // double-buffered: a call never waits for the previous call's upload
   PinBuf<int> h_chunk_off_buf[2];
   PinBuf<int> h_stream_buf[2];
   PinBuf<int> h_pset_buf[2];
+  PinBuf<RecordFrame> h_rec_buf[2];
+  PinBuf<unsigned char> h_raw;            // page-locked staging of pageable records
   cudaEvent_t tab_ev[2] = {nullptr, nullptr};
   int tab_cur = 0;
   std::vector<int> chunk_off;             // host copy of the current call's chunk table
@@ -263,8 +268,8 @@ void split_runs(pwpp_ctx* ctx, int nframes, const int32_t* streams) {
 }
 
 // Sizes the work buffers for a call over nframes frames (ctx->pt_off filled), uploads the frame tables (points, chunks,
-// stream of every frame) and splits the call into runs.
-int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_t s) {
+// stream of every frame and, for a records call, the record table) and splits the call into runs.
+int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_t s, const RecordFrame* recs = nullptr) {
   const long long total = ctx->pt_off[nframes];
   int total_chunks = 0;
   ctx->tab_cur ^= 1;
@@ -317,6 +322,13 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   CU_TRY(cudaMemcpyAsync(ctx->d_chunk_off.p, h_chunk_off.p, (nframes + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_stream.p, h_stream.p, nframes * sizeof(int), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_pset.p, h_pset.p, nframes * sizeof(int), cudaMemcpyHostToDevice, s));
+  if (recs) {
+    PinBuf<RecordFrame>& h_rec = ctx->h_rec_buf[tb];
+    CU_TRY(h_rec.reserve(nframes));
+    CU_TRY(ctx->d_rec.reserve(nframes));
+    std::memcpy(h_rec.p, recs, (size_t) nframes * sizeof(RecordFrame));
+    CU_TRY(cudaMemcpyAsync(ctx->d_rec.p, h_rec.p, nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice, s));
+  }
   CU_TRY(cudaEventRecord(ctx->tab_ev[tb], s));
   ctx->last_nframes = nframes;
   ctx->last_total = total;
@@ -566,9 +578,9 @@ int launch_runs(pwpp_ctx* ctx, int f0, int f1, size_t* r, const float4* d_pts, i
   return PWPP_OK;
 }
 
-int run_path(pwpp_ctx* ctx, int nframes, const int32_t* streams, const float4* d_pts, int has_intensity, cudaStream_t s) {
-  int rc = prepare_call(ctx, nframes, streams, s);
-  if (rc) return rc;
+// Launches the whole prepared call on stream s.
+int launch_call(pwpp_ctx* ctx, int nframes, const float4* d_pts, int has_intensity, cudaStream_t s) {
+  int rc = PWPP_OK;
   size_t r = 0;
   // per-stage timing covers one launch sequence: a call of several runs is launched, but not timed
   if (ctx->profiling) return launch_runs(ctx, 0, nframes, &r, d_pts, has_intensity, s, ctx->runs.size() == 2);
@@ -582,6 +594,12 @@ int run_path(pwpp_ctx* ctx, int nframes, const int32_t* streams, const float4* d
     f0 = f1;
   }
   return PWPP_OK;
+}
+
+int run_path(pwpp_ctx* ctx, int nframes, const int32_t* streams, const float4* d_pts, int has_intensity, cudaStream_t s) {
+  const int rc = prepare_call(ctx, nframes, streams, s);
+  if (rc) return rc;
+  return launch_call(ctx, nframes, d_pts, has_intensity, s);
 }
 
 int check_frame(pwpp_ctx* ctx, int f) {
@@ -866,6 +884,7 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   for (int c = 0; c < NUM_CLASSES; ++c) ctx->d_wq_items[c].release();
   ctx->d_out_idx.release(); ctx->d_counts.release();
   ctx->d_centers.release(); ctx->d_normals.release(); ctx->d_xyz.release();
+  ctx->d_raw.release(); ctx->d_rec.release(); ctx->h_raw.release(); for (int i = 0; i < 2; ++i) ctx->h_rec_buf[i].release();
   ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
   ctx->h_out_idx.release(); ctx->h_counts.release();
   ctx->h_centers.release(); ctx->h_normals.release();
@@ -1103,6 +1122,158 @@ int pwpp_estimate_device_xyz(pwpp_ctx* ctx, int nframes, const void* d_xyz, cons
   std::vector<int64_t> offs(h_offsets, h_offsets + nframes + 1);
   for (auto& o : offs) o -= h_offsets[0];
   return pwpp_estimate_device(ctx, nframes, ctx->d_in.p, offs.data(), 0, s);
+}
+
+// Entry of the record table for a frame of this layout whose records start at src (device memory).
+static RecordFrame record_frame(const pwpp_point_layout& L, const void* src) {
+  RecordFrame r{};
+  r.src = static_cast<const unsigned char*>(src);
+  r.step = L.point_step;
+  for (int c = 0; c < 4; ++c) { r.off[c] = L.offset[c]; r.type[c] = L.datatype[c]; }
+  if (L.offset[3] < 0) { r.off[3] = 0; r.type[3] = 0; }   // no intensity field: the kernel writes NaN
+  return r;
+}
+
+// The checks of both records entry points (include/pwpp.h), before anything is allocated or launched.
+static int check_records_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* n,
+                              const pwpp_point_layout* layouts) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  int rc = check_streams(ctx, nframes, streams);
+  if (rc) return rc;
+  std::string msg;
+  rc = check_record_layouts(nframes, frames, n, layouts, &msg);
+  if (rc) return fail(rc, msg);
+  for (int f = 0; f < nframes; ++f)
+    if (n[f] > 0x7fffffffLL - CHUNK_PTS) return fail(PWPP_ERR_INVALID_ARG, "frame " + std::to_string(f) + ": frame size out of range");
+  return PWPP_OK;
+}
+
+// Unpacks frames [f0, f1) of the prepared records call into ctx->d_in on stream s: one launch (none when the frames are empty).
+static int unpack_records(pwpp_ctx* ctx, int f0, int f1, const std::vector<RecordFrame>& recs, cudaStream_t s) {
+  if (ctx->pt_off[f1] == ctx->pt_off[f0]) return PWPP_OK;
+  const long long gx = rec_grid_x(ctx->pt_off.data() + f0, recs.data() + f0, f1 - f0);
+  k_unpack_records<<<dim3((unsigned) gx, (unsigned) (f1 - f0)), REC_THREADS, 0, s>>>(ctx->d_rec.p + f0, ctx->d_pt_off.p + f0, ctx->d_in.p);
+  ++ctx->launches;
+  CU_TRY(cudaGetLastError());
+  return PWPP_OK;
+}
+
+int pwpp_estimate_host_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* n,
+                               const pwpp_point_layout* layouts) {
+  int rc = check_records_call(ctx, nframes, streams, frames, n, layouts);
+  if (rc) return rc;
+  rc = bind_device(ctx);
+  if (rc) return rc;
+  const auto t0 = std::chrono::steady_clock::now();
+  ctx->pt_off.assign(nframes + 1, 0);
+  std::vector<long long> raw_off(nframes + 1, 0);   // every frame's records in the upload buffer, 16-byte aligned
+  for (int f = 0; f < nframes; ++f) {
+    ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
+    raw_off[f + 1] = raw_off[f] + ((n[f] * layouts[f].point_step + 15) & ~15LL);
+  }
+  const long long total = ctx->pt_off[nframes];
+  cudaStream_t s = ctx->stream, s_in = ctx->stream_h2d, s_out = ctx->stream_d2h;
+  ctx->call_times_valid = false;
+  // the buffers of the previous call must not be in flight any more (nor a device-input call on a caller's stream)
+  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  CU_TRY(cudaStreamSynchronize(s));
+  CU_TRY(cudaStreamSynchronize(s_in));
+  CU_TRY(cudaStreamSynchronize(s_out));
+  CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(total, 1)));
+  CU_TRY(ctx->d_raw.reserve((size_t) std::max<long long>(raw_off[nframes], 16)));
+  std::vector<RecordFrame> recs(nframes);
+  int has_intensity = 0;
+  for (int f = 0; f < nframes; ++f) {
+    recs[f] = record_frame(layouts[f], ctx->d_raw.p + raw_off[f]);
+    if (layouts[f].offset[3] >= 0) has_intensity = 1;
+  }
+  rc = prepare_call(ctx, nframes, streams, s, recs.data());
+  if (rc) return rc;
+  CU_TRY(ctx->h_out_idx.reserve((size_t) std::max<long long>(total, 1)));
+  CU_TRY(ctx->h_counts.reserve((size_t) 3 * nframes));
+  bool staged_any = false;
+  // the chunk pipeline of pwpp_estimate_host: H2D + unpack of chunk k+1 | kernels of chunk k | D2H of chunk k-1
+  int chunk_frames = nframes;
+  if (nframes > 1 && total > 0) {
+    const long long per_frame = std::max<long long>(1, total / nframes);
+    chunk_frames = (int) std::min<long long>(nframes, std::max<long long>(1, (4LL << 20) / per_frame));
+  }
+  const int nchunks = (nframes + chunk_frames - 1) / chunk_frames;
+  const bool one_stream = (nchunks == 1);
+  if (one_stream) { s_in = s; s_out = s; CU_TRY(cudaEventRecord(ctx->ev_begin, s)); }
+  else CU_TRY(cudaStreamWaitEvent(s_in, ctx->tab_ev[ctx->tab_cur], 0));   // the unpack reads the record table uploaded on s
+  const bool prof = ctx->profiling && nchunks == 1 && ctx->runs.size() == 2;
+  size_t run_cursor = 0;
+  for (int k = 0; k < nchunks; ++k) {
+    const int f0 = k * chunk_frames, f1 = std::min(nframes, f0 + chunk_frames);
+    for (int f = f0; f < f1; ++f) {
+      if (n[f] == 0) continue;
+      const size_t bytes = (size_t) n[f] * layouts[f].point_step;
+      bool pinned = false;
+      cudaPointerAttributes attr;
+      if (cudaPointerGetAttributes(&attr, frames[f]) == cudaSuccess) pinned = (attr.type == cudaMemoryTypeHost);
+      else cudaGetLastError();
+      const void* src = frames[f];
+      if (!pinned) {   // pageable: one memcpy into page-locked staging, then DMA
+        if (!staged_any) { CU_TRY(ctx->h_raw.reserve((size_t) std::max<long long>(raw_off[nframes], 16))); staged_any = true; }
+        std::memcpy(ctx->h_raw.p + raw_off[f], frames[f], bytes);
+        src = ctx->h_raw.p + raw_off[f];
+      }
+      CU_TRY(cudaMemcpyAsync(ctx->d_raw.p + raw_off[f], src, bytes, cudaMemcpyHostToDevice, s_in));
+    }
+    rc = unpack_records(ctx, f0, f1, recs, s_in);
+    if (rc) return rc;
+    CU_TRY(cudaEventRecord(ctx->ev0, s_in));
+    if (!one_stream) CU_TRY(cudaStreamWaitEvent(s, ctx->ev0, 0));
+    rc = launch_runs(ctx, f0, f1, &run_cursor, ctx->d_in.p, has_intensity, s, prof);
+    if (rc) return rc;
+    CU_TRY(cudaEventRecord(ctx->ev1, s));
+    if (!one_stream) CU_TRY(cudaStreamWaitEvent(s_out, ctx->ev1, 0));
+    const long long o0 = ctx->pt_off[f0], o1 = ctx->pt_off[f1];
+    for (int q = 0; q < 3; ++q)
+      CU_TRY(cudaMemcpyAsync(ctx->h_counts.p + (size_t) q * nframes + f0, ctx->d_counts.p + (size_t) q * nframes + f0, (size_t) (f1 - f0) * sizeof(int),
+                             cudaMemcpyDeviceToHost, s_out));
+    if (o1 > o0) CU_TRY(cudaMemcpyAsync(ctx->h_out_idx.p + o0, ctx->d_out_idx.p + o0, (size_t) (o1 - o0) * sizeof(int), cudaMemcpyDeviceToHost, s_out));
+  }
+  if (one_stream) CU_TRY(cudaEventRecord(ctx->ev_end, s));
+  CU_TRY(cudaStreamSynchronize(s_out));
+  CU_TRY(cudaStreamSynchronize(s));
+  ctx->call_times_valid = one_stream;
+  ctx->counts_fetched = true;
+  ctx->idx_fetched = true;
+  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
+  return PWPP_OK;
+}
+
+int pwpp_estimate_device_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* d_frames, const int64_t* n,
+                                 const pwpp_point_layout* layouts, void* cuda_stream) {
+  int rc = check_records_call(ctx, nframes, streams, d_frames, n, layouts);
+  if (rc) return rc;
+  rc = bind_device(ctx);
+  if (rc) return rc;
+  const auto t0 = std::chrono::steady_clock::now();
+  ctx->pt_off.assign(nframes + 1, 0);
+  for (int f = 0; f < nframes; ++f) ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
+  const long long total = ctx->pt_off[nframes];
+  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
+  // stream ordering of pwpp_estimate_device_xyz: the input buffer and work buffers are reused in stream order
+  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  if (!ctx->last_stream && s != ctx->stream) CU_TRY(cudaStreamSynchronize(ctx->stream));
+  CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(total, 1)));
+  std::vector<RecordFrame> recs(nframes);
+  int has_intensity = 0;
+  for (int f = 0; f < nframes; ++f) {
+    recs[f] = record_frame(layouts[f], d_frames[f]);
+    if (layouts[f].offset[3] >= 0) has_intensity = 1;
+  }
+  rc = prepare_call(ctx, nframes, streams, s, recs.data());
+  if (rc) return rc;
+  rc = unpack_records(ctx, 0, nframes, recs, s);
+  if (rc) return rc;
+  rc = launch_call(ctx, nframes, ctx->d_in.p, has_intensity, s);
+  if (rc) return rc;
+  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
+  return PWPP_OK;
 }
 
 int pwpp_device_synchronize(pwpp_ctx* ctx) {

@@ -1,6 +1,7 @@
 // pwpp_host.hpp — host-side helpers shared by the C-ABI implementation and the CPU twin used in tests.
 #pragma once
 #include <cstring>
+#include <string>
 
 #include "pwpp.h"
 #include "pwpp_gle.cuh"
@@ -53,6 +54,46 @@ inline void init_state(const pwpp_params& p, StreamState& s) {
   std::memset(&s, 0, sizeof(s));
   s.sensor_height = p.sensor_height;
   for (int i = 0; i < 4; ++i) { s.elevation_thr[i] = p.elevation_thr[i]; s.flatness_thr[i] = p.flatness_thr[i]; }
+}
+
+// bytes of a PWPP_FIELD_* datatype, 0 for an unknown code
+inline int field_bytes(int32_t datatype) {
+  static const int bytes[9] = {0, 1, 1, 2, 2, 4, 4, 4, 8};
+  return datatype >= 1 && datatype <= 8 ? bytes[datatype] : 0;
+}
+
+// The checks of pwpp_estimate_*_records on the frames, sizes and layouts of a call (include/pwpp.h), before anything is
+// allocated or launched: PWPP_OK, or the status with *msg naming the frame and the field.
+inline int check_record_layouts(int nframes, const void* const* frames, const int64_t* n, const pwpp_point_layout* layouts, std::string* msg) {
+  static const char* names[4] = {"x", "y", "z", "intensity"};
+  if (!frames || !n || !layouts) { *msg = "frames, n or layouts is NULL"; return PWPP_ERR_INVALID_ARG; }
+  for (int f = 0; f < nframes; ++f) {
+    const std::string fr = "frame " + std::to_string(f) + ": ";
+    if (n[f] < 0) { *msg = fr + "n < 0"; return PWPP_ERR_INVALID_ARG; }
+    if (n[f] > 0 && !frames[f]) { *msg = fr + "frame pointer is NULL"; return PWPP_ERR_INVALID_ARG; }
+    const pwpp_point_layout& L = layouts[f];
+    if (L.point_step < 1) { *msg = fr + "point_step " + std::to_string(L.point_step) + " < 1"; return PWPP_ERR_INVALID_ARG; }
+    if (L.point_step > PWPP_MAX_POINT_STEP) {
+      *msg = fr + "point_step " + std::to_string(L.point_step) + " > PWPP_MAX_POINT_STEP (" + std::to_string(PWPP_MAX_POINT_STEP) + ")";
+      return PWPP_ERR_UNSUPPORTED;
+    }
+    for (int c = 0; c < 4; ++c) {
+      if (c == 3 && L.offset[3] < 0) break;   // no intensity field
+      const std::string fl = fr + "field " + names[c] + ": ";
+      const int nb = field_bytes(L.datatype[c]);
+      if (nb == 0) { *msg = fl + "unknown datatype " + std::to_string(L.datatype[c]); return PWPP_ERR_INVALID_ARG; }
+      if (c < 3 && L.datatype[c] != PWPP_FIELD_FLOAT32 && L.datatype[c] != PWPP_FIELD_FLOAT64) {
+        *msg = fl + "x, y and z must be FLOAT32 or FLOAT64, got datatype " + std::to_string(L.datatype[c]);
+        return PWPP_ERR_UNSUPPORTED;
+      }
+      if (L.offset[c] < 0 || (int64_t) L.offset[c] + nb > L.point_step) {
+        *msg = fl + "bytes [" + std::to_string(L.offset[c]) + ", " + std::to_string((int64_t) L.offset[c] + nb) + ") do not fit inside point_step " +
+               std::to_string(L.point_step);
+        return PWPP_ERR_INVALID_ARG;
+      }
+    }
+  }
+  return PWPP_OK;
 }
 
 

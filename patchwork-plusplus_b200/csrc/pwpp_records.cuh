@@ -1,0 +1,137 @@
+// pwpp_records.cuh — sensor point records of any PointCloud2 layout -> the engine's packed float4 {x, y, z, intensity} points
+// (pwpp_estimate_host_records / pwpp_estimate_device_records, include/pwpp.h).
+//
+// One launch unpacks every frame of a launch range: blockIdx.y is the frame, blockIdx.x a tile of its records. The pass is
+// memory-bound (point_step bytes read and 16 written per point), so a CTA first stages its tile's contiguous byte range
+// [src + i0 * step, src + i1 * step) in shared memory: 16-byte vector loads for the 16-byte-aligned body of the range, byte loads
+// for the unaligned head and tail (at most 15 bytes each), so a 22-byte record still reads HBM in whole sectors, and no byte
+// outside the frame is touched (a caller's frame may be a view that ends anywhere). Every thread then assembles its records'
+// fields from aligned shared-memory words (funnel shifts: any field alignment), converts them to float with round-to-nearest
+// and stores one float4 per point. The datatype of a field is uniform per frame, hence per CTA: its switch does not diverge.
+#pragma once
+#include "pwpp_common.cuh"
+#include "pwpp.h"
+
+namespace pwpp {
+
+// per-frame entry of the call's record table (uploaded with the frame tables): where frame f's records are and how to read them
+struct RecordFrame {
+  const unsigned char* src;   // first byte of record 0 (device memory: the caller's buffer or the ctx's upload buffer)
+  int step;                   // point_step, 1..PWPP_MAX_POINT_STEP
+  int off[4];                 // byte offsets of x, y, z, intensity inside a record
+  int type[4];                // PWPP_FIELD_*; type[3] = 0: the frame has no intensity field (NaN intensity)
+  int pad;
+};
+static_assert(sizeof(RecordFrame) == 48, "RecordFrame is uploaded as a 48-byte record");
+
+constexpr int REC_THREADS = 256;
+constexpr int REC_TILE_BYTES = 16384;    // bytes of records one CTA stages (whole records)
+constexpr int REC_MAX_TILE_PTS = 1024;
+// shared memory: the tile, the up to 15 bytes below its first 16-byte boundary, and room for the word reads of the last field
+constexpr int REC_SMEM_WORDS = (REC_TILE_BYTES + 32) / 4;
+
+// records per CTA for a record size: 1024 for steps up to 16, 16 at the largest step
+__host__ __device__ inline int rec_tile_pts(int step) {
+  const int t = REC_TILE_BYTES / step;
+  return t < REC_MAX_TILE_PTS ? t : REC_MAX_TILE_PTS;
+}
+
+#if defined(PWPP_SIMT_EMU)
+inline float rec_i2f(int v) { return (float) v; }                 // the host's conversions round to nearest, as numpy does
+inline float rec_u2f(unsigned v) { return (float) v; }
+inline float rec_d2f(double v) { return (float) v; }
+inline double rec_lohi2d(unsigned lo, unsigned hi) { const unsigned long long b = ((unsigned long long) hi << 32) | lo; double d; std::memcpy(&d, &b, 8); return d; }
+inline void rec_ld16(void* dst, const unsigned char* p) { std::memcpy(dst, p, 16); }   // (the SIMT stand-in: a plain load)
+#else
+__device__ __forceinline__ float rec_i2f(int v) { return __int2float_rn(v); }
+__device__ __forceinline__ float rec_u2f(unsigned v) { return __uint2float_rn(v); }
+__device__ __forceinline__ float rec_d2f(double v) { return __double2float_rn(v); }
+__device__ __forceinline__ double rec_lohi2d(unsigned lo, unsigned hi) { return __hiloint2double((int) hi, (int) lo); }
+// read-once records: 16-byte load that does not allocate in L1
+__device__ __forceinline__ void rec_ld16(void* dst, const unsigned char* p) {
+  uint4 v;
+  asm("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+  *reinterpret_cast<uint4*>(dst) = v;
+}
+#endif
+
+// the 4 bytes starting at byte b of the staged words, any alignment (little-endian)
+__device__ __forceinline__ unsigned rec_word(const unsigned* s, int b) {
+  const unsigned lo = s[b >> 2], hi = s[(b >> 2) + 1];
+  return (unsigned) ((((unsigned long long) hi << 32) | lo) >> ((b & 3) * 8));
+}
+
+// FLOAT64 -> float with round-to-nearest-even; a NaN keeps its sign and the top 22 payload bits and becomes quiet (what x86's
+// conversion, and so numpy's astype(np.float32), produces; the device instruction would return the canonical NaN)
+__device__ __forceinline__ float rec_f64(unsigned lo, unsigned hi) {
+  const double d = rec_lohi2d(lo, hi);
+  if (d != d) return __uint_as_float((hi & 0x80000000u) | 0x7fc00000u | ((hi & 0x000fffffu) << 3) | (lo >> 29));
+  return rec_d2f(d);
+}
+
+__device__ __forceinline__ float rec_field(const unsigned* s, int b, int type) {
+  const unsigned w = rec_word(s, b);
+  switch (type) {
+    case PWPP_FIELD_INT8: return rec_i2f((int) (signed char) (w & 0xffu));
+    case PWPP_FIELD_UINT8: return rec_u2f(w & 0xffu);
+    case PWPP_FIELD_INT16: return rec_i2f((int) (short) (w & 0xffffu));
+    case PWPP_FIELD_UINT16: return rec_u2f(w & 0xffffu);
+    case PWPP_FIELD_INT32: return rec_i2f((int) w);
+    case PWPP_FIELD_UINT32: return rec_u2f(w);
+    case PWPP_FIELD_FLOAT32: return __uint_as_float(w);
+    case PWPP_FIELD_FLOAT64: return rec_f64(w, rec_word(s, b + 4));
+    default: return __uint_as_float(0x7fc00000u);   // no intensity field: a NaN fails every RNR test (rnr_hit)
+  }
+}
+
+// frame f = blockIdx.y of the range: records tile blockIdx.x -> dst[pt_off[f] + i]. pt_off holds absolute positions (the
+// call's frame table offset to the range's first frame).
+__global__ void __launch_bounds__(REC_THREADS) k_unpack_records(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
+                                                                 float4* __restrict__ dst) {
+  __shared__ __align__(16) unsigned s_w[REC_SMEM_WORDS];
+  const int f = blockIdx.y, tid = threadIdx.x;
+  const RecordFrame R = recs[f];
+  const long long p0 = pt_off[f];
+  const long long n = pt_off[f + 1] - p0;
+  const int tp = rec_tile_pts(R.step);
+  const long long i0 = (long long) blockIdx.x * tp;
+  if (i0 >= n) return;
+  const int cnt = (int) (n - i0 < tp ? n - i0 : tp);
+  const unsigned char* a = R.src + i0 * R.step;                 // the tile's bytes [a, b)
+  const unsigned char* b = a + (size_t) cnt * R.step;
+  const unsigned char* a_floor = (const unsigned char*) ((uintptr_t) a & ~(uintptr_t) 15);   // shared word 0 holds this address
+  const unsigned char* a16 = (const unsigned char*) (((uintptr_t) a + 15) & ~(uintptr_t) 15);
+  const unsigned char* b16 = (const unsigned char*) ((uintptr_t) b & ~(uintptr_t) 15);
+  unsigned char* s_b = reinterpret_cast<unsigned char*>(s_w);
+  if (a16 < b16) {
+    const int nvec = (int) ((b16 - a16) >> 4), vbase = (int) (a16 - a_floor);
+#pragma unroll 4
+    for (int k = tid; k < nvec; k += REC_THREADS) rec_ld16(s_b + vbase + 16 * k, a16 + 16 * k);
+    const int head = (int) (a16 - a), tail = (int) (b - b16);
+    if (tid < head) s_b[(a - a_floor) + tid] = a[tid];
+    else if (tid >= 16 && tid < 16 + tail) s_b[(b16 - a_floor) + (tid - 16)] = b16[tid - 16];
+  } else {
+    for (int k = tid; k < (int) (b - a); k += REC_THREADS) s_b[(a - a_floor) + k] = a[k];
+  }
+  __syncthreads();
+  const int r0 = (int) (a - a_floor);
+  float4* out = dst + p0 + i0;
+  for (int i = tid; i < cnt; i += REC_THREADS) {
+    const int r = r0 + i * R.step;
+    out[i] = make_float4(rec_field(s_w, r + R.off[0], R.type[0]), rec_field(s_w, r + R.off[1], R.type[1]), rec_field(s_w, r + R.off[2], R.type[2]),
+                         rec_field(s_w, r + R.off[3], R.type[3]));
+  }
+}
+
+// grid.x of a launch over frames with these sizes and steps
+inline long long rec_grid_x(const long long* pt_off, const RecordFrame* recs, int nf) {
+  long long gx = 0;
+  for (int f = 0; f < nf; ++f) {
+    const int tp = rec_tile_pts(recs[f].step);
+    const long long t = (pt_off[f + 1] - pt_off[f] + tp - 1) / tp;
+    gx = t > gx ? t : gx;
+  }
+  return gx;
+}
+
+}  // namespace pwpp

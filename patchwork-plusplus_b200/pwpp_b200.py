@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from pwpp_ctypes import PwppBinResult, PwppParams, PwppState, default_params  # noqa: F401
+from pwpp_ctypes import PwppBinResult, PwppParams, PwppPointLayout, PwppState, default_params  # noqa: F401
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PWPP_LIB") or os.path.join(_HERE, "lib", "libpwpp_b200.so")   # PWPP_LIB: a diagnostic build of the same library
@@ -41,6 +41,8 @@ def load_library():
     lib.pwpp_estimate_host_streams.argtypes = [vp, i32, vp, C.POINTER(vp), C.POINTER(i64), i32, i64, i64]
     lib.pwpp_estimate_host_streams.restype = i32
     lib.pwpp_estimate_device_streams.argtypes = [vp, i32, vp, vp, C.POINTER(i64), i32, vp]; lib.pwpp_estimate_device_streams.restype = i32
+    lib.pwpp_estimate_host_records.argtypes = [vp, i32, vp, vp, vp, vp]; lib.pwpp_estimate_host_records.restype = i32
+    lib.pwpp_estimate_device_records.argtypes = [vp, i32, vp, vp, vp, vp, vp]; lib.pwpp_estimate_device_records.restype = i32
     lib.pwpp_synchronize.argtypes = [vp]; lib.pwpp_synchronize.restype = i32
     for n in ("pwpp_num_ground", "pwpp_num_nonground"):
         getattr(lib, n).argtypes = [vp, i32]; getattr(lib, n).restype = i64
@@ -79,6 +81,38 @@ def bind_host_to_device(device: int) -> int:
 
 class PwppError(RuntimeError):
     pass
+
+
+# sensor_msgs/PointField datatype codes (PWPP_FIELD_* of include/pwpp.h) of the numpy scalar types
+FIELD_CODES = {np.dtype(np.int8): 1, np.dtype(np.uint8): 2, np.dtype(np.int16): 3, np.dtype(np.uint16): 4, np.dtype(np.int32): 5,
+               np.dtype(np.uint32): 6, np.dtype(np.float32): 7, np.dtype(np.float64): 8}
+
+
+def layout_from_dtype(dtype) -> PwppPointLayout:
+    """The record layout of a numpy structured dtype: fields `x`, `y`, `z` and optionally `intensity` (the names the reference's
+    PointCloud2 iterators use), their offsets and datatypes, and the itemsize as point_step. Fields must be scalars of native
+    (little-endian) byte order."""
+    dtype = np.dtype(dtype)
+    if dtype.fields is None:
+        raise PwppError(f"not a structured dtype: {dtype}")
+    lay = PwppPointLayout()
+    lay.point_step = dtype.itemsize
+    for c, name in enumerate(("x", "y", "z", "intensity")):
+        if name not in dtype.fields:
+            if c < 3:
+                raise PwppError(f"record dtype has no field {name!r}")
+            lay.offset[3], lay.datatype[3] = -1, 0
+            continue
+        ft, off = dtype.fields[name][:2]
+        if ft.subdtype is not None:
+            raise PwppError(f"field {name!r} has count > 1 ({ft})")
+        if not ft.isnative:
+            raise PwppError(f"field {name!r} is not in native byte order ({ft.str}); records are little-endian")
+        code = FIELD_CODES.get(ft)
+        if code is None:
+            raise PwppError(f"field {name!r} has a datatype PointCloud2 does not define ({ft})")
+        lay.offset[c], lay.datatype[c] = off, code
+    return lay
 
 
 def _check(rc):
@@ -179,6 +213,43 @@ class Engine:
                                                          C.c_void_p(stream)))
         self._n = np.diff(offsets).tolist()
         self._streams = list(range(nf)) if streams is None else [int(s) for s in streams]
+
+    def _records_call(self, fn, nf, streams, ptrs, ns, layouts, *extra):
+        ids = np.arange(nf, dtype=np.int32) if streams is None else self._stream_table(streams, nf)
+        p = (C.c_void_p * max(nf, 1))(*ptrs)
+        n = (C.c_int64 * max(nf, 1))(*ns)
+        lays = (PwppPointLayout * max(nf, 1))(*layouts)
+        _check(fn(self._h, nf, ids.ctypes.data, p, n, lays, *extra))
+        self._n = [int(k) for k in ns]
+        self._streams = ids.tolist()
+
+    def estimate_host_records(self, frames, streams=None):
+        """Sensor records of any layout from host memory (pwpp_estimate_host_records). Every frame is a 1-D structured array
+        (layout_from_dtype) or a pair (uint8 buffer, PwppPointLayout) holding len(buffer) // point_step records. `streams` as for
+        estimate_host (None: frame f on stream f)."""
+        ptrs, ns, layouts, keep = [], [], [], []
+        for fr in frames:
+            if isinstance(fr, tuple):
+                buf, lay = fr
+                buf = np.asarray(buf)
+                if buf.dtype != np.uint8 or not buf.flags.c_contiguous:
+                    raise PwppError("a (buffer, layout) frame needs a C-contiguous uint8 buffer")
+                n = buf.nbytes // lay.point_step if lay.point_step > 0 else 0
+            else:
+                buf = np.asarray(fr)
+                if buf.ndim != 1 or buf.strides[0] != buf.dtype.itemsize:
+                    raise PwppError("a structured frame must be a contiguous 1-D array of records")
+                lay, n = layout_from_dtype(buf.dtype), len(buf)
+            keep.append(buf)
+            ptrs.append(buf.ctypes.data)
+            ns.append(n)
+            layouts.append(lay)
+        self._records_call(self.lib.pwpp_estimate_host_records, len(frames), streams, ptrs, ns, layouts)
+
+    def estimate_device_records(self, ptrs, ns, layouts, streams=None, stream: int = 0):
+        """Sensor records resident on the device (pwpp_estimate_device_records): frame f is ns[f] records of layouts[f] at device
+        address ptrs[f] (any alignment), unpacked on CUDA stream `stream` (0: the ctx's own stream)."""
+        self._records_call(self.lib.pwpp_estimate_device_records, len(ptrs), streams, [int(p) for p in ptrs], ns, layouts, C.c_void_p(stream))
 
     def synchronize(self):
         _check(self.lib.pwpp_synchronize(self._h))

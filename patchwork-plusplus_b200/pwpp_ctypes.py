@@ -46,3 +46,8 @@ class PwppState(C.Structure):
 class PwppBinResult(C.Structure):
     _fields_ = [("mean", C.c_double * 3), ("normal", C.c_double * 3), ("sv", C.c_double * 3), ("d", C.c_double),
                 ("n", C.c_int32), ("n_ground", C.c_int32), ("verdict", C.c_int32), ("fitted", C.c_int32)]
+
+
+class PwppPointLayout(C.Structure):
+    """Mirror of `pwpp_point_layout` (include/pwpp.h): the record layout of a frame for pwpp_estimate_*_records."""
+    _fields_ = [("point_step", C.c_int32), ("offset", C.c_int32 * 4), ("datatype", C.c_int32 * 4)]
