@@ -5,6 +5,7 @@
 
 No torch, no JIT cache: plain nvcc / g++ invocations.
 """
+import glob
 import os
 import subprocess
 import sys
@@ -27,7 +28,6 @@ def _newer(target, sources):
 def build_core(force=False, verbose=False):
     os.makedirs(LIB, exist_ok=True)
     src = os.path.join(HERE, "csrc", "pwpp_capi.cu")
-    import glob
     deps = glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]
     out = os.path.join(LIB, "libpwpp_b200.so")
     if force or _newer(out, deps):
@@ -81,6 +81,12 @@ def build_examples(force=False):
     if force or _newer(out4, [src4, hdr, os.path.join(REPO, "include", "patchwork", "pointcloud2.hpp"), core]):
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + os.path.join(REPO, "include"), src4, "-o", out4,
                                "-L" + LIB, "-lpwpp_b200", "-Wl,-rpath,$ORIGIN"])
+    # the record unpack kernel alone, compiled for sm_90a like the core (GPU cases of tests/test_simt_records.py)
+    src5 = os.path.join(REPO, "tests", "gpu_records_probe.cu")
+    out5 = os.path.join(LIB, "libpwpp_records_probe.so")
+    if force or _newer(out5, [src5] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out5, src5])
     return out
 
 

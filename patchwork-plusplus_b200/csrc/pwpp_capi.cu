@@ -1124,16 +1124,6 @@ int pwpp_estimate_device_xyz(pwpp_ctx* ctx, int nframes, const void* d_xyz, cons
   return pwpp_estimate_device(ctx, nframes, ctx->d_in.p, offs.data(), 0, s);
 }
 
-// Entry of the record table for a frame of this layout whose records start at src (device memory).
-static RecordFrame record_frame(const pwpp_point_layout& L, const void* src) {
-  RecordFrame r{};
-  r.src = static_cast<const unsigned char*>(src);
-  r.step = L.point_step;
-  for (int c = 0; c < 4; ++c) { r.off[c] = L.offset[c]; r.type[c] = L.datatype[c]; }
-  if (L.offset[3] < 0) { r.off[3] = 0; r.type[3] = 0; }   // no intensity field: the kernel writes NaN
-  return r;
-}
-
 // The checks of both records entry points (include/pwpp.h), before anything is allocated or launched.
 static int check_records_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* n,
                               const pwpp_point_layout* layouts) {

@@ -43,6 +43,7 @@ inline void build_geometry(const pwpp_params& p, Geometry& g, AlgoParams& ap, bo
   g.f_max_range = (float) g.max_range;
   g.nbins = g.bin_base[4];
   ap.RNR_ver_angle_thr = p.RNR_ver_angle_thr; ap.RNR_intensity_thr = p.RNR_intensity_thr;
+  ap.f_RNR_intensity_thr = float_ru(p.RNR_intensity_thr);
   ap.th_seeds = p.th_seeds; ap.th_seeds_v = p.th_seeds_v; ap.th_dist = p.th_dist; ap.th_dist_v = p.th_dist_v;
   ap.uprightness_thr = p.uprightness_thr; ap.adaptive_seed_selection_margin = p.adaptive_seed_selection_margin;
   ap.num_iter = p.num_iter; ap.num_lpr = p.num_lpr; ap.num_min_pts = p.num_min_pts; ap.num_rings_of_interest = p.num_rings_of_interest;

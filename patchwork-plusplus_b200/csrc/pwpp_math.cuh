@@ -127,7 +127,9 @@ struct AlgoParams {
   int num_iter, num_lpr, num_min_pts, num_rings_of_interest;
   int enable_RNR, enable_RVPF, enable_TGR;
   int max_flatness_storage, max_elevation_storage;
+  float f_RNR_intensity_thr;   // float_ru(RNR_intensity_thr): rnr_hit's intensity test in fp32, exact
 };
+static_assert(sizeof(AlgoParams) == 104, "f_RNR_intensity_thr sits in what was tail padding: AlgoParamSets keeps its size");
 
 // Pseudo-bins after the nbins real ones (see include/pwpp.h pwpp_copy_bin_ids)
 #define PW_BIN_RNR(nb) ((nb))        /* reflected noise, S:391-396 -> nonground            */
@@ -138,10 +140,9 @@ struct AlgoParams {
 // reflected_noise_removal predicate, S:385-391. r is computed in float like the reference does.
 PW_HD bool rnr_hit(float x, float y, float z, float intensity, double sensor_height, const AlgoParams& ap) {
   // cheap conjuncts first (pure predicates, order does not matter): S:391
-  if (!(intensity < (float) ap.RNR_intensity_thr + 1e-3f)) return false;   // float pre-filter, exact test below
+  if (!(intensity < ap.f_RNR_intensity_thr)) return false;   // (double) intensity < RNR_intensity_thr (float_ru)
   const double zd = (double) z;
   if (!(zd < dsub(-sensor_height, 0.8))) return false;
-  if (!((double) intensity < ap.RNR_intensity_thr)) return false;
   const float rf = fsqrt(fadd(fmul(x, x), fmul(y, y)));          // S:387 (float ops, std::sqrt(float))
   const double ang = ddiv(dmul(atan2_exact(zd, (double) rf), 180.0), PW_PI);  // S:389
   return ang < ap.RNR_ver_angle_thr;

@@ -62,7 +62,7 @@ __device__ __forceinline__ unsigned rec_word(const unsigned* s, int b) {
 }
 
 // FLOAT64 -> float with round-to-nearest-even; a NaN keeps its sign and the top 22 payload bits and becomes quiet (what x86's
-// conversion, and so numpy's astype(np.float32), produces; the device instruction would return the canonical NaN)
+// conversion, and so numpy's astype(np.float32), produces; the H100's instruction alone gave the same bits on every NaN tested: the branch makes it a rule)
 __device__ __forceinline__ float rec_f64(unsigned lo, unsigned hi) {
   const double d = rec_lohi2d(lo, hi);
   if (d != d) return __uint_as_float((hi & 0x80000000u) | 0x7fc00000u | ((hi & 0x000fffffu) << 3) | (lo >> 29));
@@ -121,6 +121,16 @@ __global__ void __launch_bounds__(REC_THREADS) k_unpack_records(const RecordFram
     out[i] = make_float4(rec_field(s_w, r + R.off[0], R.type[0]), rec_field(s_w, r + R.off[1], R.type[1]), rec_field(s_w, r + R.off[2], R.type[2]),
                          rec_field(s_w, r + R.off[3], R.type[3]));
   }
+}
+
+// Entry of the record table for a frame of this (validated) layout whose records start at src (device memory).
+inline RecordFrame record_frame(const pwpp_point_layout& L, const void* src) {
+  RecordFrame r{};
+  r.src = static_cast<const unsigned char*>(src);
+  r.step = L.point_step;
+  for (int c = 0; c < 4; ++c) { r.off[c] = L.offset[c]; r.type[c] = L.datatype[c]; }
+  if (L.offset[3] < 0) { r.off[3] = 0; r.type[3] = 0; }   // no intensity field: the kernel writes NaN
+  return r;
 }
 
 // grid.x of a launch over frames with these sizes and steps
