@@ -105,7 +105,7 @@ class PatchWorkpp {
   ~PatchWorkpp() { if (ctx_) pwpp_destroy(ctx_); }
   PatchWorkpp(const PatchWorkpp&) = delete;
   PatchWorkpp& operator=(const PatchWorkpp&) = delete;
-  PatchWorkpp(PatchWorkpp&& o) noexcept : params_(o.params_), ctx_(o.ctx_), n_(o.n_), ran_(o.ran_) { o.ctx_ = nullptr; }
+  PatchWorkpp(PatchWorkpp&& o) noexcept : params_(o.params_), ctx_(o.ctx_), n_(o.n_), ran_(o.ran_), step_(o.step_) { o.ctx_ = nullptr; }
 
   // reference :152 for raw buffers: element (i,c) of the N x cols cloud is data[i*row_stride + c*col_stride].
   void estimateGround(const float* data, int64_t n, int cols, int64_t row_stride, int64_t col_stride) {
@@ -116,6 +116,7 @@ class PatchWorkpp {
     check(pwpp_estimate_host(ctx_, 1, ptrs, ns, cols >= 4 ? 4 : 3, row_stride, col_stride));
     n_ = n;
     ran_ = true;
+    step_ = 0;
   }
 
   // Device-resident cloud (zero-copy path, SURVEY 8f-1): packed N x 4 {x,y,z,intensity} or N x 3 rows in device memory.
@@ -130,6 +131,7 @@ class PatchWorkpp {
     if (!stream) check(pwpp_device_synchronize(ctx_));
     n_ = n;
     ran_ = true;
+    step_ = 0;
   }
   // Sensor records of any PointCloud2 layout (pwpp_estimate_host_records / pwpp_estimate_device_records): n records of
   // layout.point_step bytes at `data`, unpacked on the GPU. on_device: `data` is device memory, with the stream rules of
@@ -148,6 +150,7 @@ class PatchWorkpp {
     }
     n_ = n;
     ran_ = true;
+    step_ = (size_t) layout.point_step;
   }
   // device views of the last call's index lists (int32, valid until the next estimateGround*): {pointer, count}
   std::pair<const int32_t*, int64_t> groundIndicesDevice() {
@@ -173,6 +176,11 @@ class PatchWorkpp {
   std::vector<float> getNongroundVec() { std::vector<float> v(3 * (size_t) count(pwpp_num_nonground(ctx_, 0))); if (!v.empty()) check(pwpp_copy_nonground_xyz(ctx_, 0, v.data())); return v; }
   std::vector<float> getCentersVec() { std::vector<float> v(3 * (size_t) count(pwpp_num_patches(ctx_, 0))); if (!v.empty()) check(pwpp_copy_centers(ctx_, 0, v.data())); return v; }
   std::vector<float> getNormalsVec() { std::vector<float> v(3 * (size_t) count(pwpp_num_patches(ctx_, 0))); if (!v.empty()) check(pwpp_copy_normals(ctx_, 0, v.data())); return v; }
+  // Ground / non-ground points of the last estimateGroundRecords() as whole records of its layout, byte for byte (every field
+  // the sensor sent): count * point_step bytes (pwpp_copy_ground_records / pwpp_copy_nonground_records). Throws after a call
+  // that did not take records.
+  std::vector<uint8_t> getGroundRecords() { return records(true); }
+  std::vector<uint8_t> getNongroundRecords() { return records(false); }
 
 #ifdef PATCHWORKPP_HAVE_EIGEN
   // the reference's exact signatures (:152, :157-163)
@@ -198,8 +206,15 @@ class PatchWorkpp {
   pwpp_ctx* ctx_ = nullptr;
   int64_t n_ = 0;
   bool ran_ = false;
+  size_t step_ = 0;   // point_step of the last estimateGroundRecords() (0 after any other call)
 
   static void check(int rc) { if (rc != PWPP_OK) throw std::runtime_error(std::string("PatchWorkpp: ") + pwpp_last_error()); }
+  std::vector<uint8_t> records(bool ground) {
+    check(pwpp_host_record_results(ctx_, nullptr, nullptr));   // (fails, with its message, when the last call did not take records)
+    std::vector<uint8_t> v((size_t) count(ground ? pwpp_num_ground(ctx_, 0) : pwpp_num_nonground(ctx_, 0)) * step_);
+    if (!v.empty()) check(ground ? pwpp_copy_ground_records(ctx_, 0, v.data()) : pwpp_copy_nonground_records(ctx_, 0, v.data()));
+    return v;
+  }
   // before the first estimateGround() the reference's getters return empty matrices (its members are empty): a count
   // of -1 with nothing processed yet is 0 here, any other failure throws
   int64_t count(int64_t c) const { if (c < 0) { if (!ran_) return 0; throw std::runtime_error(std::string("PatchWorkpp: ") + pwpp_last_error()); } return c; }

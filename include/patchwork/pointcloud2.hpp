@@ -116,5 +116,26 @@ inline PointCloud2Payload makeCloudPayload(PatchWorkpp& pw, bool ground) {
   return p;
 }
 
+// Payload of an outgoing PointCloud2 in the INPUT's own layout: the ground (ground = true) or non-ground points of the last
+// estimateGround(pw, in) as whole records, byte for byte (intensity, ring, per-point time, padding: every field the sensor
+// sent, which the reference node's x/y/z messages drop), gathered on the GPU. The message takes in.point_step and in.fields,
+// height 1, width = the count. `in` describes the message of that call (its data is not read again).
+struct PointCloud2RecordsPayload {
+  std::vector<uint8_t> data;
+  uint32_t width = 0, height = 1, point_step = 0, row_step = 0;
+  bool is_bigendian = false;
+  std::vector<PointField> fields;
+};
+inline PointCloud2RecordsPayload makeRecordsPayload(PatchWorkpp& pw, bool ground, const PointCloud2Message& in) {
+  PointCloud2RecordsPayload p;
+  p.data = ground ? pw.getGroundRecords() : pw.getNongroundRecords();
+  p.point_step = in.point_step;
+  p.fields = in.fields;
+  p.is_bigendian = in.is_bigendian;
+  p.width = in.point_step ? (uint32_t) (p.data.size() / in.point_step) : 0;
+  p.row_step = p.width * p.point_step;
+  return p;
+}
+
 }  // namespace patchwork
 #endif

@@ -236,9 +236,31 @@ typedef struct pwpp_point_layout {
 int pwpp_estimate_host_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames,
                                const int64_t* n, const pwpp_point_layout* layouts /* [nframes] */);
 /* Device-resident records: unpacked on `cuda_stream` (NULL = the ctx's own stream) with the stream-ordering rules of
- * pwpp_estimate_device_xyz; the records must stay untouched until the call's work on that stream has run. */
+ * pwpp_estimate_device_xyz; the records must stay untouched until the call's work on that stream has run, and, when the
+ * record results below are wanted, until they have been fetched (their gather reads the caller's buffers). */
 int pwpp_estimate_device_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* d_frames,
                                  const int64_t* n, const pwpp_point_layout* layouts /* [nframes] */, void* cuda_stream);
+
+/* Results of the last RECORDS call (pwpp_estimate_*_records) as records of each frame's own layout: every field the sensor
+ * sent (intensity, ring, per-point time, padding) comes back byte for byte, so a ROS 2 node can publish its ground and
+ * non-ground clouds with the input's fields. Frame f's region starts at byte h_offsets[f] (16-byte aligned; h_offsets has
+ * nframes + 1 entries): num_ground(f) ground records, then num_nonground(f) non-ground records, in index-list order (record k
+ * is input record k of the frame's lists, PWPP_ORDER_BIN or PWPP_ORDER_REFERENCE as the call ran); the bytes after them in
+ * the region are unspecified.
+ *   - The first of these four functions called after a call gathers the records of every frame in one kernel on the GPU
+ *     (pwpp_launch_count rises by one; none for a call without points), on the call's stream; later calls of them reuse it.
+ *     The host view adds one device->host copy into a page-locked buffer, and the per-frame getters copy from that. Calls
+ *     that never ask for record results allocate and launch nothing for them.
+ *   - Host blocking of pwpp_device_record_results: none once its buffers are warm, i.e. after a request of a call at least as
+ *     large (in frames and record bytes). A request that first reserves or grows the output buffers or their page-locked
+ *     offset table allocates device / page-locked memory, which the CUDA runtime may synchronize; and a request waits for the
+ *     previous request's offset-table upload to have run (enqueued one call earlier, so in practice long done).
+ *   - PWPP_ERR_INVALID_ARG before any call, for a frame outside the last call, and when the last call did not take records
+ *     (the xyz getters serve those). Valid until the next estimate call. */
+int pwpp_device_record_results(pwpp_ctx* ctx, const void** d_records, const int64_t** h_offsets);  /* enqueued on the call's stream; no host sync once warm */
+int pwpp_host_record_results(pwpp_ctx* ctx, const void** h_records, const int64_t** h_offsets);    /* page-locked view, one D2H */
+int pwpp_copy_ground_records(pwpp_ctx* ctx, int f, void* dst);       /* num_ground(f) * point_step bytes */
+int pwpp_copy_nonground_records(pwpp_ctx* ctx, int f, void* dst);    /* num_nonground(f) * point_step bytes */
 
 /* cudaDeviceSynchronize() on the ctx's device: what a binding calls before handing device memory produced on an unknown
  * stream to pwpp_estimate_device (and what makes its results visible to every stream afterwards). */

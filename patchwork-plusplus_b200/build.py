@@ -81,12 +81,23 @@ def build_examples(force=False):
     if force or _newer(out4, [src4, hdr, os.path.join(REPO, "include", "patchwork", "pointcloud2.hpp"), core]):
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + os.path.join(REPO, "include"), src4, "-o", out4,
                                "-L" + LIB, "-lpwpp_b200", "-Wl,-rpath,$ORIGIN"])
+    src7 = os.path.join(REPO, "tests", "pc2_records_out_driver.cpp")   # makeRecordsPayload against the real engine (GPU test)
+    out7 = os.path.join(LIB, "pc2_records_out_driver")
+    if force or _newer(out7, [src7, hdr, os.path.join(REPO, "include", "patchwork", "pointcloud2.hpp"), core]):
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + os.path.join(REPO, "include"), src7, "-o", out7,
+                               "-L" + LIB, "-lpwpp_b200", "-Wl,-rpath,$ORIGIN"])
     # the record unpack kernel alone, compiled for sm_90a like the core (GPU cases of tests/test_simt_records.py)
     src5 = os.path.join(REPO, "tests", "gpu_records_probe.cu")
     out5 = os.path.join(LIB, "libpwpp_records_probe.so")
     if force or _newer(out5, [src5] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out5, src5])
+    # the record gather kernel alone, the same way (GPU cases of tests/test_records_gather_backends.py)
+    src6 = os.path.join(REPO, "tests", "gpu_records_gather_probe.cu")
+    out6 = os.path.join(LIB, "libpwpp_records_gather_probe.so")
+    if force or _newer(out6, [src6] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out6, src6])
     return out
 
 

@@ -51,13 +51,14 @@ int fail(int code, const std::string& msg) {
 
 unsigned long long g_alloc_gen = 0;   // bumped whenever a device buffer moves: captured CUDA graphs hold the old pointers
 
-template <typename T>
+// InGraphs = false: a buffer no captured launch sequence reads (its moves leave the graphs valid)
+template <typename T, bool InGraphs = true>
 struct DevBuf {
   T* p = nullptr;
   size_t cap = 0;  // elements
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
-    ++g_alloc_gen;
+    if (InGraphs) ++g_alloc_gen;
     if (p) cudaFree(p);
     p = nullptr;
     cap = 0;
@@ -166,6 +167,9 @@ struct pwpp_ctx {
   DevBuf<float> d_xyz;            // gather scratch
   DevBuf<unsigned char> d_raw;    // pwpp_estimate_host_records: the frames' records as uploaded, unpacked on the device
   DevBuf<RecordFrame> d_rec;      // [F] record table of a records call
+  // record results (pwpp_*_record_results), reserved by the first call that asks for them
+  DevBuf<unsigned char, false> d_rec_out;   // every frame's ground and non-ground records, region f at rec_off[f]
+  DevBuf<long long, false> d_rec_off;       // [F+1]
 
   PinBuf<float4> h_in;
   PinBuf<long long> h_pt_off_buf[2];      // double-buffered: a call never waits for the previous call's upload
@@ -174,6 +178,9 @@ struct pwpp_ctx {
   PinBuf<int> h_pset_buf[2];
   PinBuf<RecordFrame> h_rec_buf[2];
   PinBuf<unsigned char> h_raw;            // page-locked staging of pageable records
+  PinBuf<long long> h_rec_off;            // upload of rec_off; ev_rec_off marks when the copy has read it
+  PinBuf<unsigned char> h_rec_out;        // host view of d_rec_out
+  cudaEvent_t ev_rec_off = nullptr;
   cudaEvent_t tab_ev[2] = {nullptr, nullptr};
   int tab_cur = 0;
   std::vector<int> chunk_off;             // host copy of the current call's chunk table
@@ -193,6 +200,9 @@ struct pwpp_ctx {
   std::vector<long long> pt_off;  // host copy
   const float4* last_pts = nullptr;  // device pointer of the input of the last call
   bool counts_fetched = false, idx_fetched = false, patches_fetched = false;
+  std::vector<RecordFrame> last_recs;     // record table of the last call when it took records (empty otherwise)
+  std::vector<long long> rec_off;         // [F+1] byte offsets of the record result regions (set by the gather)
+  bool rec_gathered = false, rec_fetched = false;
   double last_time_us = 0.0;
   cudaStream_t last_stream = nullptr;
 
@@ -322,6 +332,9 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   CU_TRY(cudaMemcpyAsync(ctx->d_chunk_off.p, h_chunk_off.p, (nframes + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_stream.p, h_stream.p, nframes * sizeof(int), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_pset.p, h_pset.p, nframes * sizeof(int), cudaMemcpyHostToDevice, s));
+  if (recs) ctx->last_recs.assign(recs, recs + nframes);
+  else ctx->last_recs.clear();
+  ctx->rec_gathered = ctx->rec_fetched = false;
   if (recs) {
     PinBuf<RecordFrame>& h_rec = ctx->h_rec_buf[tb];
     CU_TRY(h_rec.reserve(nframes));
@@ -885,6 +898,8 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   ctx->d_out_idx.release(); ctx->d_counts.release();
   ctx->d_centers.release(); ctx->d_normals.release(); ctx->d_xyz.release();
   ctx->d_raw.release(); ctx->d_rec.release(); ctx->h_raw.release(); for (int i = 0; i < 2; ++i) ctx->h_rec_buf[i].release();
+  ctx->d_rec_out.release(); ctx->d_rec_off.release(); ctx->h_rec_off.release(); ctx->h_rec_out.release();
+  if (ctx->ev_rec_off) cudaEventDestroy(ctx->ev_rec_off);
   ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
   ctx->h_out_idx.release(); ctx->h_counts.release();
   ctx->h_centers.release(); ctx->h_normals.release();
@@ -1265,6 +1280,83 @@ int pwpp_estimate_device_records(pwpp_ctx* ctx, int nframes, const int32_t* stre
   ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
   return PWPP_OK;
 }
+
+// Record results of the last call: the first request gathers every frame's records into d_rec_out on the call's stream (one
+// launch, none when the call had no points), and no later request of the same call gathers again. The host blocks only where
+// a buffer is first reserved or grows, and on the previous request's offset-table upload (include/pwpp.h).
+static int gather_records(pwpp_ctx* ctx) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (ctx->last_nframes <= 0) return fail(PWPP_ERR_INVALID_ARG, "no estimate call yet");
+  if (ctx->last_recs.empty()) return fail(PWPP_ERR_INVALID_ARG, "the last estimate call did not take records (pwpp_estimate_host_records / pwpp_estimate_device_records)");
+  if (ctx->rec_gathered) return PWPP_OK;
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const int nf = ctx->last_nframes;
+  cudaStream_t s = ctx->last_stream;
+  ctx->rec_off.assign(nf + 1, 0);
+  rec_out_offsets(ctx->pt_off.data(), ctx->last_recs.data(), nf, ctx->rec_off.data());
+  CU_TRY(ctx->d_rec_out.reserve((size_t) std::max<long long>(ctx->rec_off[nf], 16)));
+  CU_TRY(ctx->d_rec_off.reserve(nf + 1));
+  if (ctx->ev_rec_off) CU_TRY(cudaEventSynchronize(ctx->ev_rec_off));   // the previous gather's upload has read the staging
+  else CU_TRY(cudaEventCreateWithFlags(&ctx->ev_rec_off, cudaEventDisableTiming));
+  CU_TRY(ctx->h_rec_off.reserve(nf + 1));
+  std::memcpy(ctx->h_rec_off.p, ctx->rec_off.data(), (size_t) (nf + 1) * sizeof(long long));
+  CU_TRY(cudaMemcpyAsync(ctx->d_rec_off.p, ctx->h_rec_off.p, (size_t) (nf + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+  CU_TRY(cudaEventRecord(ctx->ev_rec_off, s));
+  if (ctx->last_total > 0) {
+    const long long gx = rec_grid_x(ctx->pt_off.data(), ctx->last_recs.data(), nf);
+    k_gather_records<<<dim3((unsigned) gx, (unsigned) nf), REC_THREADS, 0, s>>>(ctx->d_rec.p, ctx->d_pt_off.p, ctx->d_rec_off.p, ctx->d_counts.p + 2 * nf,
+                                                                               ctx->d_out_idx.p, ctx->d_rec_out.p);
+    ++ctx->launches;
+    CU_TRY(cudaGetLastError());
+  }
+  ctx->rec_gathered = true;
+  return PWPP_OK;
+}
+
+// The gathered records in the page-locked host view (one D2H per call), and the counts.
+static int fetch_records(pwpp_ctx* ctx) {
+  int rc = gather_records(ctx);
+  if (rc) return rc;
+  rc = fetch_counts(ctx);
+  if (rc) return rc;
+  if (ctx->rec_fetched) return PWPP_OK;
+  const long long bytes = ctx->rec_off[ctx->last_nframes];
+  CU_TRY(ctx->h_rec_out.reserve((size_t) std::max<long long>(bytes, 16)));
+  if (bytes > 0) CU_TRY(cudaMemcpyAsync(ctx->h_rec_out.p, ctx->d_rec_out.p, (size_t) bytes, cudaMemcpyDeviceToHost, ctx->last_stream));
+  CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  ctx->rec_fetched = true;
+  return PWPP_OK;
+}
+
+int pwpp_device_record_results(pwpp_ctx* ctx, const void** d_records, const int64_t** h_offsets) {
+  const int rc = gather_records(ctx);
+  if (rc) return rc;
+  if (d_records) *d_records = ctx->d_rec_out.p;
+  if (h_offsets) *h_offsets = reinterpret_cast<const int64_t*>(ctx->rec_off.data());
+  return PWPP_OK;
+}
+int pwpp_host_record_results(pwpp_ctx* ctx, const void** h_records, const int64_t** h_offsets) {
+  const int rc = fetch_records(ctx);
+  if (rc) return rc;
+  if (h_records) *h_records = ctx->h_rec_out.p;
+  if (h_offsets) *h_offsets = reinterpret_cast<const int64_t*>(ctx->rec_off.data());
+  return PWPP_OK;
+}
+static int copy_records(pwpp_ctx* ctx, int f, void* dst, bool ground) {
+  int rc = check_frame(ctx, f);
+  if (rc) return rc;
+  rc = fetch_records(ctx);
+  if (rc) return rc;
+  const long long step = ctx->last_recs[f].step;
+  const int ng = ctx->h_counts.p[f];
+  const int nn = frame_n(ctx, f) - ng - count_of(ctx, 2, f);
+  const long long cnt = ground ? ng : nn;
+  if (cnt > 0) std::memcpy(dst, ctx->h_rec_out.p + ctx->rec_off[f] + (ground ? 0 : (long long) ng * step), (size_t) (cnt * step));
+  return PWPP_OK;
+}
+int pwpp_copy_ground_records(pwpp_ctx* ctx, int f, void* dst) { return copy_records(ctx, f, dst, true); }
+int pwpp_copy_nonground_records(pwpp_ctx* ctx, int f, void* dst) { return copy_records(ctx, f, dst, false); }
 
 int pwpp_device_synchronize(pwpp_ctx* ctx) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");

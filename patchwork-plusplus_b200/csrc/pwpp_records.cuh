@@ -144,4 +144,164 @@ inline long long rec_grid_x(const long long* pt_off, const RecordFrame* recs, in
   return gx;
 }
 
+// ---- the way back: the segmented lists as whole records of each frame's own layout (pwpp_*_record_results) ----------------
+//
+// k_gather_records writes, for every frame f of a call, output record k (0 <= k < ng + nn) = input record idx[pt_off[f] + k],
+// byte for byte, to dst + rec_off[f] + k * step: the ground list, then the non-ground list, as k_emit left them. The dropped
+// count (ng + nn = n - dropped) comes from the device (the call's count row), so the host sizes the grid from n[f] alone and
+// CTAs past ng + nn return at once. A CTA assembles a tile of whole output records (rec_tile_pts) in shared memory, laid out at the
+// tile's own distance from a 16-byte boundary of dst: every thread builds aligned shared words from the frame's records with
+// aligned 4-byte loads (a 64-bit shift re-aligns them: a funnel shift), byte loads where a word would reach outside the frame,
+// then the tile goes out with 16-byte stores for its aligned body and byte stores for its head and tail (at most 15 bytes each).
+// The sources of a tile are scattered and each word's address depends on a shared-memory load of its record's index, so a
+// thread issues the loads of REC_GW words before it assembles any of them: memory-level parallelism, not bandwidth, is what
+// a gather of 4-byte words runs out of first.
+// No byte outside [src, src + n * step) is read and none outside [rec_off[f], rec_off[f] + (ng + nn) * step) is written.
+
+#if defined(PWPP_SIMT_EMU)
+inline unsigned rec_ld4(const unsigned char* p) { unsigned v; std::memcpy(&v, p, 4); return v; }
+inline void rec_st16(unsigned char* p, const void* src) { std::memcpy(p, src, 16); }
+#else
+__device__ __forceinline__ unsigned rec_ld4(const unsigned char* p) { return __ldg(reinterpret_cast<const unsigned*>(p)); }
+// written once, read by the caller's D2H or kernels: a streaming store
+__device__ __forceinline__ void rec_st16(unsigned char* p, const void* src) { __stcs(reinterpret_cast<uint4*>(p), *reinterpret_cast<const uint4*>(src)); }
+#endif
+
+constexpr int REC_GW = 4;   // words a thread of k_gather_records has in flight (two aligned loads per record piece)
+
+// the 4 bytes at p of the frame, one at a time; bytes at or beyond hi read as 0 (the frame's first or last bytes)
+__device__ __forceinline__ unsigned rec_bytes4(const unsigned char* p, const unsigned char* hi) {
+  unsigned v = 0;
+  for (int k = 0; k < 4 && p + k < hi; ++k) v |= (unsigned) p[k] << (8 * k);
+  return v;
+}
+__device__ __forceinline__ unsigned rec_low_bytes(unsigned u, int len) { return len >= 4 ? u : (u & ((1u << (8 * len)) - 1u)); }
+
+// the 4 bytes at p (any alignment) of the frame [lo, hi); bytes at or beyond hi read as 0 (p >= lo)
+__device__ __forceinline__ unsigned rec_src4(const unsigned char* p, const unsigned char* lo, const unsigned char* hi) {
+  const unsigned char* a = (const unsigned char*) ((uintptr_t) p & ~(uintptr_t) 3);
+  const int sh = (int) ((uintptr_t) p & 3) * 8;
+  if (a >= lo && a + (sh ? 8 : 4) <= hi) {
+    const unsigned w0 = rec_ld4(a), w1 = sh ? rec_ld4(a + 4) : 0u;
+    return (unsigned) ((((unsigned long long) w1 << 32) | w0) >> sh);
+  }
+  return rec_bytes4(p, hi);
+}
+
+// frame f = blockIdx.y: output records [k0, k0 + tile) of its region. recs / pt_off / rec_off / nd are the call's tables (the
+// unpack's record table, point offsets, byte offsets of the output regions, dropped counts), idx the index lists.
+__global__ void __launch_bounds__(REC_THREADS, 4) k_gather_records(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
+                                                                 const long long* __restrict__ rec_off, const int* __restrict__ nd,
+                                                                 const int* __restrict__ idx,
+                                                                 unsigned char* __restrict__ dst) {
+  __shared__ __align__(16) unsigned s_w[REC_SMEM_WORDS];
+  __shared__ int s_idx[REC_MAX_TILE_PTS];
+  const int f = blockIdx.y, tid = threadIdx.x;
+  const long long p0 = pt_off[f];
+  const long long n = pt_off[f + 1] - p0;
+  const long long m = n - nd[f];                       // ground + non-ground records of the frame
+  const int step = recs[f].step;
+  const int tp = rec_tile_pts(step);
+  const long long k0 = (long long) blockIdx.x * tp;
+  if (k0 >= m) return;
+  const int cnt = (int) (m - k0 < tp ? m - k0 : tp);
+  const unsigned char* lo = recs[f].src;
+  const unsigned char* hi = lo + n * step;
+  for (int i = tid; i < cnt; i += REC_THREADS) s_idx[i] = idx[p0 + k0 + i];
+  unsigned char* a = dst + rec_off[f] + k0 * step;          // the tile's bytes [a, b) of dst
+  unsigned char* b = a + (size_t) cnt * step;
+  unsigned char* a_floor = (unsigned char*) ((uintptr_t) a & ~(uintptr_t) 15);   // shared word 0 stands for this address
+  const int r0 = (int) (a - a_floor), r1 = r0 + cnt * step;   // the tile's bytes in shared memory
+  __syncthreads();
+  // shared word w: tile bytes t = 4w + j - r0 (r0 <= 4w + j < r1), byte t % step of source record s_idx[t / step]
+  const int w_beg = r0 >> 2, w_end = (r1 + 3) >> 2;
+  if (step < 4) {
+    // a word may hold bytes of up to four records: one piece per record it touches
+    for (int w = w_beg + tid; w < w_end; w += REC_THREADS) {
+      int j = r0 - 4 * w > 0 ? r0 - 4 * w : 0;
+      const int je = r1 - 4 * w < 4 ? r1 - 4 * w : 4;
+      const int t = 4 * w + j - r0;
+      int i = t / step, c = t - i * step;
+      unsigned v = 0;
+      while (j < je) {
+        const int len = je - j < step - c ? je - j : step - c;
+        v |= rec_low_bytes(rec_src4(lo + (long long) s_idx[i] * step + c, lo, hi), len) << (8 * j);
+        j += len;
+        ++i;
+        c = 0;
+      }
+      s_w[w] = v;
+    }
+  } else {
+    // step >= 4: a word holds piece A (record i from its byte c) and, where records meet, piece B (record i + 1 from byte 0).
+    // Pass 1 issues the two aligned loads of every piece of REC_GW words (predicated off where they would leave the frame);
+    // pass 2 re-aligns and combines them, with byte loads for the pieces at the frame's two ends.
+    for (int wb = w_beg + tid; wb < w_end; wb += REC_GW * REC_THREADS) {
+      unsigned la0[REC_GW], la1[REC_GW], lb0[REC_GW], lb1[REC_GW];
+      const unsigned char* pa[REC_GW];
+      const unsigned char* pb[REC_GW];
+      int ja[REC_GW], na[REC_GW], nb[REC_GW];
+      bool oka[REC_GW], okb[REC_GW];
+#pragma unroll
+      for (int q = 0; q < REC_GW; ++q) {
+        const int w = wb + q * REC_THREADS;
+        int i = 0, c = 0, j0 = 0, je = 0;
+        if (w < w_end) {
+          j0 = r0 - 4 * w > 0 ? r0 - 4 * w : 0;
+          je = r1 - 4 * w < 4 ? r1 - 4 * w : 4;
+          const int t = 4 * w + j0 - r0;
+          i = t / step;
+          c = t - i * step;
+        }
+        ja[q] = j0;
+        na[q] = je - j0 < step - c ? je - j0 : step - c;   // 0 past the tile
+        nb[q] = je - j0 - na[q];
+        pa[q] = lo + (long long) s_idx[i] * step + c;
+        pb[q] = nb[q] > 0 ? lo + (long long) s_idx[i + 1] * step : lo;
+        const unsigned char* a4 = (const unsigned char*) ((uintptr_t) pa[q] & ~(uintptr_t) 3);
+        const unsigned char* b4 = (const unsigned char*) ((uintptr_t) pb[q] & ~(uintptr_t) 3);
+        oka[q] = na[q] > 0 && a4 >= lo && a4 + 8 <= hi;
+        okb[q] = nb[q] > 0 && b4 >= lo && b4 + 8 <= hi;
+        la0[q] = oka[q] ? rec_ld4(a4) : 0u;
+        la1[q] = oka[q] ? rec_ld4(a4 + 4) : 0u;
+        lb0[q] = okb[q] ? rec_ld4(b4) : 0u;
+        lb1[q] = okb[q] ? rec_ld4(b4 + 4) : 0u;
+      }
+#pragma unroll
+      for (int q = 0; q < REC_GW; ++q) {
+        const int w = wb + q * REC_THREADS;
+        if (w >= w_end) continue;
+        const int sa = (int) ((uintptr_t) pa[q] & 3) * 8, sb = (int) ((uintptr_t) pb[q] & 3) * 8;
+        const unsigned ua = oka[q] ? (unsigned) ((((unsigned long long) la1[q] << 32) | la0[q]) >> sa) : rec_bytes4(pa[q], hi);
+        unsigned v = rec_low_bytes(ua, na[q]) << (8 * ja[q]);
+        if (nb[q] > 0) {
+          const unsigned ub = okb[q] ? (unsigned) ((((unsigned long long) lb1[q] << 32) | lb0[q]) >> sb) : rec_bytes4(pb[q], hi);
+          v |= rec_low_bytes(ub, nb[q]) << (8 * (ja[q] + na[q]));
+        }
+        s_w[w] = v;
+      }
+    }
+  }
+  __syncthreads();
+  const unsigned char* s_b = reinterpret_cast<const unsigned char*>(s_w);
+  unsigned char* a16 = (unsigned char*) (((uintptr_t) a + 15) & ~(uintptr_t) 15);
+  unsigned char* b16 = (unsigned char*) ((uintptr_t) b & ~(uintptr_t) 15);
+  if (a16 < b16) {
+    const int nvec = (int) ((b16 - a16) >> 4), vbase = (int) (a16 - a_floor);
+#pragma unroll 4
+    for (int k = tid; k < nvec; k += REC_THREADS) rec_st16(a16 + 16 * k, s_b + vbase + 16 * k);
+    const int head = (int) (a16 - a), tail = (int) (b - b16);
+    if (tid < head) a[tid] = s_b[r0 + tid];
+    else if (tid >= 16 && tid < 16 + tail) b16[tid - 16] = s_b[(b16 - a_floor) + (tid - 16)];
+  } else {
+    for (int k = tid; k < (int) (b - a); k += REC_THREADS) a[k] = s_b[r0 + k];
+  }
+}
+
+// Byte offsets of every frame's output region (16-byte aligned, room for all n[f] records): off[nf + 1].
+inline void rec_out_offsets(const long long* pt_off, const RecordFrame* recs, int nf, long long* off) {
+  off[0] = 0;
+  for (int f = 0; f < nf; ++f) off[f + 1] = off[f] + (((pt_off[f + 1] - pt_off[f]) * recs[f].step + 15) & ~15LL);
+}
+
 }  // namespace pwpp

@@ -44,6 +44,10 @@ def load_library():
     lib.pwpp_estimate_host_records.argtypes = [vp, i32, vp, vp, vp, vp]; lib.pwpp_estimate_host_records.restype = i32
     lib.pwpp_estimate_device_records.argtypes = [vp, i32, vp, vp, vp, vp, vp]; lib.pwpp_estimate_device_records.restype = i32
     lib.pwpp_synchronize.argtypes = [vp]; lib.pwpp_synchronize.restype = i32
+    lib.pwpp_device_record_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_device_record_results.restype = i32
+    lib.pwpp_host_record_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_host_record_results.restype = i32
+    for n in ("pwpp_copy_ground_records", "pwpp_copy_nonground_records"):
+        getattr(lib, n).argtypes = [vp, i32, vp]; getattr(lib, n).restype = i32
     for n in ("pwpp_num_ground", "pwpp_num_nonground"):
         getattr(lib, n).argtypes = [vp, i32]; getattr(lib, n).restype = i64
     for n in ("pwpp_copy_ground_indices", "pwpp_copy_nonground_indices", "pwpp_copy_ground_xyz", "pwpp_copy_nonground_xyz",
@@ -150,6 +154,7 @@ class Engine:
         self.nbins = self.lib.pwpp_num_bins(h)   # with several sets: the largest bin count of the sets
         self._n = []
         self._streams = []   # stream of every frame of the last call
+        self._rec_dtypes = []   # record dtype of every frame of the last records call (uint8 rows of point_step for (buffer, layout) frames)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -191,6 +196,7 @@ class Engine:
             _check(self.lib.pwpp_estimate_host_streams(self._h, nf, ids.ctypes.data, ptrs, ns, cols, cols, 1))
         self._n = [f.shape[0] for f in frames]
         self._streams = list(range(nf)) if streams is None else [int(s) for s in streams]
+        self._rec_dtypes = []
 
     def estimate_host_strided(self, ptrs, ns, cols, row_stride, col_stride):
         nf = len(ptrs)
@@ -198,6 +204,7 @@ class Engine:
         n = (C.c_int64 * nf)(*ns)
         self._n = list(ns)
         self._streams = list(range(nf))
+        self._rec_dtypes = []
         _check(self.lib.pwpp_estimate_host(self._h, nf, p, n, cols, row_stride, col_stride))
 
     def estimate_device(self, d_ptr: int, offsets, has_intensity: bool = True, stream: int = 0, streams=None):
@@ -213,21 +220,25 @@ class Engine:
                                                          C.c_void_p(stream)))
         self._n = np.diff(offsets).tolist()
         self._streams = list(range(nf)) if streams is None else [int(s) for s in streams]
+        self._rec_dtypes = []
 
-    def _records_call(self, fn, nf, streams, ptrs, ns, layouts, *extra):
+    def _records_call(self, fn, nf, streams, ptrs, ns, layouts, *extra, dtypes=None):
         ids = np.arange(nf, dtype=np.int32) if streams is None else self._stream_table(streams, nf)
         p = (C.c_void_p * max(nf, 1))(*ptrs)
         n = (C.c_int64 * max(nf, 1))(*ns)
         lays = (PwppPointLayout * max(nf, 1))(*layouts)
+        self._rec_dtypes = []
         _check(fn(self._h, nf, ids.ctypes.data, p, n, lays, *extra))
         self._n = [int(k) for k in ns]
         self._streams = ids.tolist()
+        self._rec_dtypes = [dt if dt is not None else np.dtype((np.uint8, (lay.point_step,)))
+                            for dt, lay in zip(dtypes or [None] * nf, layouts)]
 
     def estimate_host_records(self, frames, streams=None):
         """Sensor records of any layout from host memory (pwpp_estimate_host_records). Every frame is a 1-D structured array
         (layout_from_dtype) or a pair (uint8 buffer, PwppPointLayout) holding len(buffer) // point_step records. `streams` as for
         estimate_host (None: frame f on stream f)."""
-        ptrs, ns, layouts, keep = [], [], [], []
+        ptrs, ns, layouts, keep, dtypes = [], [], [], [], []
         for fr in frames:
             if isinstance(fr, tuple):
                 buf, lay = fr
@@ -235,21 +246,26 @@ class Engine:
                 if buf.dtype != np.uint8 or not buf.flags.c_contiguous:
                     raise PwppError("a (buffer, layout) frame needs a C-contiguous uint8 buffer")
                 n = buf.nbytes // lay.point_step if lay.point_step > 0 else 0
+                dtypes.append(None)
             else:
                 buf = np.asarray(fr)
                 if buf.ndim != 1 or buf.strides[0] != buf.dtype.itemsize:
                     raise PwppError("a structured frame must be a contiguous 1-D array of records")
                 lay, n = layout_from_dtype(buf.dtype), len(buf)
+                dtypes.append(buf.dtype)
             keep.append(buf)
             ptrs.append(buf.ctypes.data)
             ns.append(n)
             layouts.append(lay)
-        self._records_call(self.lib.pwpp_estimate_host_records, len(frames), streams, ptrs, ns, layouts)
+        self._records_call(self.lib.pwpp_estimate_host_records, len(frames), streams, ptrs, ns, layouts, dtypes=dtypes)
 
-    def estimate_device_records(self, ptrs, ns, layouts, streams=None, stream: int = 0):
+    def estimate_device_records(self, ptrs, ns, layouts, streams=None, stream: int = 0, dtypes=None):
         """Sensor records resident on the device (pwpp_estimate_device_records): frame f is ns[f] records of layouts[f] at device
-        address ptrs[f] (any alignment), unpacked on CUDA stream `stream` (0: the ctx's own stream)."""
-        self._records_call(self.lib.pwpp_estimate_device_records, len(ptrs), streams, [int(p) for p in ptrs], ns, layouts, C.c_void_p(stream))
+        address ptrs[f] (any alignment), unpacked on CUDA stream `stream` (0: the ctx's own stream). `dtypes`: optional record dtype
+        of every frame, the dtype ground_records / nonground_records return (default: uint8 rows of point_step). The buffers must
+        stay untouched until the record results are fetched, when they are wanted."""
+        self._records_call(self.lib.pwpp_estimate_device_records, len(ptrs), streams, [int(p) for p in ptrs], ns, layouts, C.c_void_p(stream),
+                           dtypes=dtypes)
 
     def synchronize(self):
         _check(self.lib.pwpp_synchronize(self._h))
@@ -275,6 +291,50 @@ class Engine:
 
     def nonground_xyz(self, f=0):
         n = self.num_nonground(f); return self._get(self.lib.pwpp_copy_nonground_xyz, f, n, np.float32, (n, 3))
+
+    def _records(self, fn, f, n):
+        if not 0 <= f < len(self._rec_dtypes):   # (no records call, or a bad f: the C-ABI reports it)
+            _check(fn(self._h, f, None))
+        dt = self._rec_dtypes[f]
+        out = np.empty(n, dtype=dt)
+        if n > 0:
+            _check(fn(self._h, f, out.ctypes.data))
+        return out
+
+    def ground_records(self, f=0):
+        """Ground points of frame f of the last records call as whole input records, byte for byte (every field the sensor sent):
+        an array of the frame's structured dtype, or (count, point_step) uint8 for a (buffer, layout) frame."""
+        return self._records(self.lib.pwpp_copy_ground_records, f, self.num_ground(f))
+
+    def nonground_records(self, f=0):
+        return self._records(self.lib.pwpp_copy_nonground_records, f, self.num_nonground(f))
+
+    def device_record_lists(self):
+        """Zero-copy view of the last records call's record results on the device: (records, offsets) with records a torch uint8
+        CUDA tensor and offsets int64[nframes + 1] (numpy). Frame f's region starts at byte offsets[f]: num_ground(f) ground
+        records, then num_nonground(f) non-ground records of its point_step. The gather is enqueued on the call's stream: the
+        caller synchronizes with it (or Engine.synchronize()). Valid until the next estimate call."""
+        import torch
+        a, b = C.c_void_p(), C.c_void_p()
+        _check(self.lib.pwpp_device_record_results(self._h, C.byref(a), C.byref(b)))
+        nf = len(self._n)
+        off = np.ctypeslib.as_array((C.c_int64 * (nf + 1)).from_address(b.value)).copy()
+        total = int(off[-1])
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr, n):
+                self.__cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (ptr, False), "version": 3, "strides": None}
+        rec = torch.as_tensor(_View(a.value, total), device="cuda") if total > 0 else torch.empty(0, dtype=torch.uint8, device="cuda")
+        return rec, off
+
+    def host_record_lists(self):
+        """The same in the page-locked host view (one device->host copy): (records uint8[total] numpy view, offsets int64[nframes + 1])."""
+        a, b = C.c_void_p(), C.c_void_p()
+        _check(self.lib.pwpp_host_record_results(self._h, C.byref(a), C.byref(b)))
+        nf = len(self._n)
+        off = np.ctypeslib.as_array((C.c_int64 * (nf + 1)).from_address(b.value)).copy()
+        rec = np.ctypeslib.as_array((C.c_uint8 * max(int(off[-1]), 1)).from_address(a.value))[:int(off[-1])]
+        return rec, off
 
     def num_patches(self, f=0): return int(self.lib.pwpp_num_patches(self._h, f))
 
