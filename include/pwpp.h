@@ -262,6 +262,59 @@ int pwpp_host_record_results(pwpp_ctx* ctx, const void** h_records, const int64_
 int pwpp_copy_ground_records(pwpp_ctx* ctx, int f, void* dst);       /* num_ground(f) * point_step bytes */
 int pwpp_copy_nonground_records(pwpp_ctx* ctx, int f, void* dst);    /* num_nonground(f) * point_step bytes */
 
+/* ---- bound calls: frame sizes read on the GPU, capturable into the caller's CUDA graph --------------------------------------
+ * A GPU pipeline often knows a frame's size only on the device (a compaction kernel wrote it, or a static-shape pipeline pads
+ * every frame to a capacity and carries the count as a device tensor). A ctx holds at most one BOUND call: its frames, their
+ * capacities, the device array of their counts and the stream table, fixed once by pwpp_bind_call. Running it needs only a
+ * CUDA stream, performs no host synchronisation, and may be captured into the caller's CUDA graph; every run or replay reads
+ * the current counts and frame contents.
+ *
+ * pwpp_bind_call: frame f is up to max_n[f] records of layouts[f] at device address frames[f] (any alignment, as in
+ * pwpp_estimate_device_records), of stream streams[f]. Its size is d_counts[f] (device int64[nframes]), read by the GPU when
+ * the call runs. Does all host work now: the checks of the records entry points (with n = max_n: the message names the
+ * frame), the stream-table checks and the run split, and reserving every work buffer for sum(max_n) points. It uploads the
+ * stream, set and record tables into buffers the bound call owns, then synchronizes. Binding ends the previous call's results
+ * (the buffers they live in may move). PWPP_ERR_INVALID_ARG also when a call is already bound or d_counts is NULL.
+ *
+ * pwpp_run_bound_call: enqueues the bound call on cuda_stream (NULL = the ctx's own stream). Only kernels, device-to-device
+ * work and event record / wait between the ctx's streams: no host synchronisation, no allocation and no host-memory copy. It
+ * may be captured into a CUDA graph (global capture mode included); replays then read the current counts and frames. The
+ * run makes the bound call the ctx's last call.
+ *
+ * pwpp_bound_call_results: device views of the bound call's results, at fixed addresses while it stays bound, laid out like
+ * pwpp_device_results with the offsets on the device: *d_offsets int64[nframes + 1] (the exclusive scan of the accepted
+ * counts: frame f's region of *d_indices starts there), *d_num_ground int32[nframes], *d_status int32[nframes]. Calling it
+ * also makes the bound call the ctx's last call, so the per-frame host getters (pwpp_num_ground, pwpp_copy_*_indices,
+ * centers, normals, bin results and ids, pwpp_host_results) serve its results after a run or a graph replay; they fetch the
+ * offsets with their first device->host copy. After a replay the caller synchronizes with the replay's stream before using
+ * the host getters (they only synchronize with the stream of the last pwpp_run_bound_call).
+ *
+ * Rules:
+ *   - Out-of-range counts. A count outside [0, max_n[f]] cannot return an error from a replay: frame f runs as an empty
+ *     frame instead, exactly as a direct call with n = 0 would, its stream state advances as after that empty call, and
+ *     d_status[f] = PWPP_COUNT_OUT_OF_RANGE (0 otherwise). The other frames are unaffected. Nothing past
+ *     frames[f] + max_n[f] * point_step is ever read.
+ *   - Buffers are frozen while a call is bound, so no buffer a captured graph holds ever moves:
+ *       a direct call that would grow a work buffer returns PWPP_ERR_CAPACITY before anything runs, and no state changes
+ *       (a direct call that fits runs as usual);
+ *       pwpp_set_output_order returns PWPP_ERR_INVALID_ARG: the bound call keeps the order it was bound with.
+ *     pwpp_unbind_call lifts the freeze and makes graphs that hold the bound call invalid.
+ *   - Shared state and results. Direct calls and runs of the bound call use the same stream state and the same result
+ *     buffers; each one's results are valid until the next call or replay. The caller orders replays against direct calls
+ *     (same stream, or its own events): the ctx cannot see a replay, and a capture cannot wait on an event recorded outside it.
+ *   - pwpp_launch_count rises, per pwpp_run_bound_call, by one table launch, one unpack launch when any max_n > 0, and the
+ *     usual launch sequence of each run (grids sized for the capacities).
+ *   - The record results (pwpp_*_record_results, pwpp_copy_*_records) refuse a bound call with a message: their gather
+ *     needs host offsets. */
+#define PWPP_COUNT_OUT_OF_RANGE 1   /* d_status[f]: d_counts[f] < 0 or > max_n[f]; the frame was run as an empty frame */
+int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
+                   const pwpp_point_layout* layouts, const int64_t* d_counts);
+int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream);
+int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int64_t** d_offsets, const int32_t** d_num_ground,
+                            const int32_t** d_status);
+/* Releases the bound call (PWPP_ERR_INVALID_ARG when none is bound). Its results stay readable until the next call. */
+int pwpp_unbind_call(pwpp_ctx* ctx);
+
 /* cudaDeviceSynchronize() on the ctx's device: what a binding calls before handing device memory produced on an unknown
  * stream to pwpp_estimate_device (and what makes its results visible to every stream afterwards). */
 int pwpp_device_synchronize(pwpp_ctx* ctx);

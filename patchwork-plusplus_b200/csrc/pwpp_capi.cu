@@ -205,6 +205,21 @@ struct pwpp_ctx {
   bool rec_gathered = false, rec_fetched = false;
   double last_time_us = 0.0;
   cudaStream_t last_stream = nullptr;
+  bool last_bound = false, off_fetched = false;   // the last call is the bound call; its point offsets were fetched (fetch_offsets)
+
+  // the bound call (pwpp_bind_call): what its runs re-establish and launch. The work buffers are frozen while it is bound.
+  struct Bound {
+    bool on = false;
+    int nf = 0, has_intensity = 0;
+    const long long* d_counts = nullptr;    // the caller's device counts
+    long long unpack_gx = 0;                // grid.x of the unpack, from the capacities
+    std::vector<int> runs, frame_set, run_chunks, cap_chunk_off;   // run_chunks[r]: the run's largest ceil(max_n / CHUNK_PTS)
+    std::vector<long long> cap_pt_off;      // the capacity layout: sizes grids and picks the dense front end only
+  } bound;
+  DevBuf<long long, false> d_bmax;        // [F] max_n
+  DevBuf<int, false> d_bstream, d_bpset;  // [F] the bound call's stream and set tables
+  DevBuf<int, false> d_bstatus;           // [F] PWPP_COUNT_OUT_OF_RANGE or 0
+  DevBuf<RecordFrame, false> d_brec;      // [F] its record table
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
   struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
@@ -277,6 +292,54 @@ void split_runs(pwpp_ctx* ctx, int nframes, const int32_t* streams) {
   for (int f = 0; f < nframes; ++f) ctx->last_pos[streams[f]] = -1;
 }
 
+// The work buffers of a call over nframes frames, total points and total_chunks chunks (and the input buffer, with_input).
+// With check_only nothing is allocated: PWPP_ERR_CAPACITY when one of them would have to grow (frozen by a bound call).
+int reserve_work(pwpp_ctx* ctx, int nframes, long long total, long long total_chunks, bool with_input, bool check_only) {
+  const size_t nb = ctx->gs.nbs, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO, nf = (size_t) nframes, np = (size_t) total;
+  bool grow = false;
+  cudaError_t err = cudaSuccess;
+  auto need = [&](auto& b, size_t n) {
+    if (check_only) grow = grow || n > b.cap;
+    else if (err == cudaSuccess) err = b.reserve(n);
+  };
+  if (with_input) need(ctx->d_in, std::max<size_t>(np, 1));
+  need(ctx->d_pt_off, nf + 1);
+  need(ctx->d_chunk_off, nf + 1);
+  need(ctx->d_stream, nf);
+  need(ctx->d_pset, nf);
+  need(ctx->d_bin_ids, np);
+  need(ctx->d_chist, (size_t) total_chunks * nbp);
+  need(ctx->d_cbase, (size_t) total_chunks * nbp);
+  need(ctx->d_bin_off, nf * (nbp + 1));
+  need(ctx->d_sorted, np);
+  need(ctx->d_part, np);
+  if (ctx->order_mode) need(ctx->d_labels, np);
+  need(ctx->d_fits, nf * nb);
+  need(ctx->d_segs, nf * nb_all);
+  for (int c = 0; c < NUM_CLASSES; ++c) need(ctx->d_wq_items[c], nf * nb);
+  need(ctx->d_out_idx, np);
+  need(ctx->d_counts, 3 * nf);
+  need(ctx->d_centers, nf * nb * 3);
+  need(ctx->d_normals, nf * nb * 3);
+  if (grow)
+    return fail(PWPP_ERR_CAPACITY, "a call of " + std::to_string(nframes) + " frames and " + std::to_string(total) +
+                                       " points does not fit the work buffers frozen by the bound call (pwpp_unbind_call lifts the freeze)");
+  if (err != cudaSuccess) return fail(PWPP_ERR_CUDA, std::string("reserving the work buffers: ") + cudaGetErrorString(err));
+  return PWPP_OK;
+}
+
+// A direct call while a call is bound: PWPP_ERR_CAPACITY, before anything runs or changes, when the call would grow a work
+// buffer. Frame f has n[f] points (negative sizes were refused by the caller).
+int check_frozen(pwpp_ctx* ctx, int nframes, const int64_t* n, bool with_input) {
+  if (!ctx->bound.on) return PWPP_OK;
+  long long total = 0, chunks = 0;
+  for (int f = 0; f < nframes; ++f) {
+    total += n[f];
+    chunks += (n[f] + CHUNK_PTS - 1) / CHUNK_PTS;
+  }
+  return reserve_work(ctx, nframes, total, chunks, with_input, true);
+}
+
 // Sizes the work buffers for a call over nframes frames (ctx->pt_off filled), uploads the frame tables (points, chunks,
 // stream of every frame and, for a records call, the record table) and splits the call into runs.
 int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_t s, const RecordFrame* recs = nullptr) {
@@ -309,25 +372,8 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   h_pt_off.p[nframes] = total;
   h_chunk_off.p[nframes] = total_chunks;
   ctx->chunk_off[nframes] = total_chunks;
-  const int nb = ctx->gs.nbs, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO;
-  CU_TRY(ctx->d_pt_off.reserve(nframes + 1));
-  CU_TRY(ctx->d_chunk_off.reserve(nframes + 1));
-  CU_TRY(ctx->d_stream.reserve(nframes));
-  CU_TRY(ctx->d_pset.reserve(nframes));
-  CU_TRY(ctx->d_bin_ids.reserve((size_t) total));
-  CU_TRY(ctx->d_chist.reserve((size_t) total_chunks * nbp));
-  CU_TRY(ctx->d_cbase.reserve((size_t) total_chunks * nbp));
-  CU_TRY(ctx->d_bin_off.reserve((size_t) nframes * (nbp + 1)));
-  CU_TRY(ctx->d_sorted.reserve((size_t) total));
-  CU_TRY(ctx->d_part.reserve((size_t) total));
-  if (ctx->order_mode) CU_TRY(ctx->d_labels.reserve((size_t) total));
-  CU_TRY(ctx->d_fits.reserve((size_t) nframes * nb));
-  CU_TRY(ctx->d_segs.reserve((size_t) nframes * nb_all));
-  for (int c = 0; c < NUM_CLASSES; ++c) CU_TRY(ctx->d_wq_items[c].reserve((size_t) nframes * nb));
-  CU_TRY(ctx->d_out_idx.reserve((size_t) total));
-  CU_TRY(ctx->d_counts.reserve((size_t) 3 * nframes));
-  CU_TRY(ctx->d_centers.reserve((size_t) nframes * nb * 3));
-  CU_TRY(ctx->d_normals.reserve((size_t) nframes * nb * 3));
+  const int rc = reserve_work(ctx, nframes, total, total_chunks, false, false);
+  if (rc) return rc;
   CU_TRY(cudaMemcpyAsync(ctx->d_pt_off.p, h_pt_off.p, (nframes + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_chunk_off.p, h_chunk_off.p, (nframes + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
   CU_TRY(cudaMemcpyAsync(ctx->d_stream.p, h_stream.p, nframes * sizeof(int), cudaMemcpyHostToDevice, s));
@@ -345,6 +391,7 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   CU_TRY(cudaEventRecord(ctx->tab_ev[tb], s));
   ctx->last_nframes = nframes;
   ctx->last_total = total;
+  ctx->last_bound = false;
   ctx->counts_fetched = ctx->idx_fetched = ctx->patches_fetched = false;
   ctx->stage_valid = false;
   return PWPP_OK;
@@ -621,9 +668,25 @@ int check_frame(pwpp_ctx* ctx, int f) {
   return PWPP_OK;
 }
 
+// The bound call's point offsets (the device scan of its accepted counts) into the host description of the last call.
+int fetch_offsets(pwpp_ctx* ctx) {
+  if (!ctx->last_bound || ctx->off_fetched) return PWPP_OK;
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const int nf = ctx->last_nframes;
+  ctx->pt_off.assign(nf + 1, 0);
+  CU_TRY(cudaMemcpyAsync(ctx->pt_off.data(), ctx->d_pt_off.p, (size_t) (nf + 1) * sizeof(long long), cudaMemcpyDeviceToHost, ctx->last_stream));
+  CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  ctx->last_total = ctx->pt_off[nf];
+  ctx->off_fetched = true;
+  return PWPP_OK;
+}
+
 int fetch_counts(pwpp_ctx* ctx) {
   if (ctx->counts_fetched) return PWPP_OK;
-  int rc = bind_device(ctx);
+  int rc = fetch_offsets(ctx);
+  if (rc) return rc;
+  rc = bind_device(ctx);
   if (rc) return rc;
   CU_TRY(ctx->h_counts.reserve((size_t) 3 * ctx->last_nframes));
   CU_TRY(cudaMemcpyAsync(ctx->h_counts.p, ctx->d_counts.p, (size_t) 3 * ctx->last_nframes * sizeof(int), cudaMemcpyDeviceToHost, ctx->last_stream));
@@ -899,6 +962,7 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   ctx->d_centers.release(); ctx->d_normals.release(); ctx->d_xyz.release();
   ctx->d_raw.release(); ctx->d_rec.release(); ctx->h_raw.release(); for (int i = 0; i < 2; ++i) ctx->h_rec_buf[i].release();
   ctx->d_rec_out.release(); ctx->d_rec_off.release(); ctx->h_rec_off.release(); ctx->h_rec_out.release();
+  ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
   if (ctx->ev_rec_off) cudaEventDestroy(ctx->ev_rec_off);
   ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
   ctx->h_out_idx.release(); ctx->h_counts.release();
@@ -965,7 +1029,9 @@ static int estimate_host_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams
   if (cols != 3 && cols != 4) return fail(PWPP_ERR_INVALID_ARG, "cols must be 3 or 4 (x,y,z[,intensity])");
   for (int f = 0; f < nframes; ++f)
     if (n[f] < 0 || (n[f] > 0 && !pts[f])) return fail(PWPP_ERR_INVALID_ARG, "bad frame pointer/size");
-  int rc = bind_device(ctx);
+  int rc = check_frozen(ctx, nframes, n, true);
+  if (rc) return rc;
+  rc = bind_device(ctx);
   if (rc) return rc;
   const auto t0 = std::chrono::steady_clock::now();
   ctx->pt_off.assign(nframes + 1, 0);
@@ -1090,7 +1156,14 @@ static int estimate_device_impl(pwpp_ctx* ctx, int nframes, const int32_t* strea
   for (int f = 1; f <= nframes; ++f)
     if (h_offsets[f] < h_offsets[f - 1]) return fail(PWPP_ERR_INVALID_ARG, "offsets must be non-decreasing");
   if (h_offsets[nframes] > h_offsets[0] && !d_pts) return fail(PWPP_ERR_INVALID_ARG, "d_pts is NULL");
-  int rc = bind_device(ctx);
+  int rc = PWPP_OK;
+  if (ctx->bound.on) {
+    std::vector<int64_t> sizes(nframes);
+    for (int f = 0; f < nframes; ++f) sizes[f] = h_offsets[f + 1] - h_offsets[f];
+    rc = check_frozen(ctx, nframes, sizes.data(), false);
+    if (rc) return rc;
+  }
+  rc = bind_device(ctx);
   if (rc) return rc;
   const auto t0 = std::chrono::steady_clock::now();
   ctx->pt_off.assign(nframes + 1, 0);
@@ -1126,6 +1199,12 @@ int pwpp_estimate_device_xyz(pwpp_ctx* ctx, int nframes, const void* d_xyz, cons
   if (rc) return rc;
   const long long total = h_offsets[nframes] - h_offsets[0];
   if (total < 0 || (total > 0 && !d_xyz)) return fail(PWPP_ERR_INVALID_ARG, "bad offsets / d_xyz is NULL");
+  if (ctx->bound.on) {
+    std::vector<int64_t> sizes(nframes);
+    for (int f = 0; f < nframes; ++f) sizes[f] = h_offsets[f + 1] - h_offsets[f];
+    rc = check_frozen(ctx, nframes, sizes.data(), true);
+    if (rc) return rc;
+  }
   cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
   if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
   if (!ctx->last_stream && s != ctx->stream) CU_TRY(cudaStreamSynchronize(ctx->stream));
@@ -1153,6 +1232,14 @@ static int check_records_call(pwpp_ctx* ctx, int nframes, const int32_t* streams
   return PWPP_OK;
 }
 
+// The checks of a direct records call: those above, and the freeze of a bound call.
+static int check_direct_records_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* n,
+                                     const pwpp_point_layout* layouts) {
+  const int rc = check_records_call(ctx, nframes, streams, frames, n, layouts);
+  if (rc) return rc;
+  return check_frozen(ctx, nframes, n, true);
+}
+
 // Unpacks frames [f0, f1) of the prepared records call into ctx->d_in on stream s: one launch (none when the frames are empty).
 static int unpack_records(pwpp_ctx* ctx, int f0, int f1, const std::vector<RecordFrame>& recs, cudaStream_t s) {
   if (ctx->pt_off[f1] == ctx->pt_off[f0]) return PWPP_OK;
@@ -1165,7 +1252,7 @@ static int unpack_records(pwpp_ctx* ctx, int f0, int f1, const std::vector<Recor
 
 int pwpp_estimate_host_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* n,
                                const pwpp_point_layout* layouts) {
-  int rc = check_records_call(ctx, nframes, streams, frames, n, layouts);
+  int rc = check_direct_records_call(ctx, nframes, streams, frames, n, layouts);
   if (rc) return rc;
   rc = bind_device(ctx);
   if (rc) return rc;
@@ -1252,7 +1339,7 @@ int pwpp_estimate_host_records(pwpp_ctx* ctx, int nframes, const int32_t* stream
 
 int pwpp_estimate_device_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* d_frames, const int64_t* n,
                                  const pwpp_point_layout* layouts, void* cuda_stream) {
-  int rc = check_records_call(ctx, nframes, streams, d_frames, n, layouts);
+  int rc = check_direct_records_call(ctx, nframes, streams, d_frames, n, layouts);
   if (rc) return rc;
   rc = bind_device(ctx);
   if (rc) return rc;
@@ -1281,12 +1368,144 @@ int pwpp_estimate_device_records(pwpp_ctx* ctx, int nframes, const int32_t* stre
   return PWPP_OK;
 }
 
+// ---- the bound call (include/pwpp.h) ----
+
+// Makes the bound call the ctx's last call, run on stream s: the host getters fetch its offsets first (fetch_offsets).
+static void make_bound_last(pwpp_ctx* ctx, cudaStream_t s) {
+  const pwpp_ctx::Bound& b = ctx->bound;
+  ctx->last_nframes = b.nf;
+  ctx->frame_set = b.frame_set;
+  ctx->last_recs.clear();
+  ctx->last_pts = ctx->d_in.p;
+  ctx->last_stream = s;
+  ctx->last_total = 0;
+  ctx->last_bound = true;
+  ctx->off_fetched = ctx->counts_fetched = ctx->idx_fetched = ctx->patches_fetched = false;
+  ctx->rec_gathered = ctx->rec_fetched = false;
+  ctx->stage_valid = ctx->call_times_valid = false;
+}
+
+int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
+                   const pwpp_point_layout* layouts, const int64_t* d_counts) {
+  int rc = check_records_call(ctx, nframes, streams, frames, max_n, layouts);
+  if (rc) return rc;
+  if (ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "a call is already bound (pwpp_unbind_call releases it)");
+  if (!d_counts) return fail(PWPP_ERR_INVALID_ARG, "d_counts is NULL");
+  pwpp_ctx::Bound b;
+  b.nf = nframes;
+  b.d_counts = reinterpret_cast<const long long*>(d_counts);
+  b.cap_pt_off.assign(nframes + 1, 0);
+  b.cap_chunk_off.assign(nframes + 1, 0);
+  long long chunks = 0;
+  for (int f = 0; f < nframes; ++f) {
+    b.cap_pt_off[f + 1] = b.cap_pt_off[f] + max_n[f];
+    chunks += (max_n[f] + CHUNK_PTS - 1) / CHUNK_PTS;
+    if (chunks > 0x7fffffffLL) return fail(PWPP_ERR_INVALID_ARG, "frame " + std::to_string(f) + ": the capacities exceed 2^31 - 1 chunks of " + std::to_string(CHUNK_PTS) + " points");
+    b.cap_chunk_off[f + 1] = (int) chunks;
+  }
+  std::vector<RecordFrame> recs(nframes);
+  for (int f = 0; f < nframes; ++f) {
+    recs[f] = record_frame(layouts[f], frames[f]);
+    if (layouts[f].offset[3] >= 0) b.has_intensity = 1;
+    b.frame_set.push_back(ctx->stream_set[streams[f]]);
+  }
+  b.unpack_gx = b.cap_pt_off[nframes] > 0 ? rec_grid_x(b.cap_pt_off.data(), recs.data(), nframes) : 0;
+  split_runs(ctx, nframes, streams);
+  b.runs = ctx->runs;
+  for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
+    int m = 0;
+    for (int f = b.runs[r]; f < b.runs[r + 1]; ++f) m = std::max(m, b.cap_chunk_off[f + 1] - b.cap_chunk_off[f]);
+    b.run_chunks.push_back(m);
+  }
+  rc = bind_device(ctx);
+  if (rc) return rc;
+  // the buffers may move: whatever the ctx enqueued before has finished with them, and the last call's results end here
+  if (ctx->last_stream) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  CU_TRY(cudaStreamSynchronize(ctx->stream));
+  ctx->last_nframes = 0;
+  ctx->last_bound = false;
+  rc = reserve_work(ctx, nframes, b.cap_pt_off[nframes], chunks, true, false);
+  if (rc) return rc;
+  CU_TRY(ctx->d_bmax.reserve(nframes));
+  CU_TRY(ctx->d_bstream.reserve(nframes));
+  CU_TRY(ctx->d_bpset.reserve(nframes));
+  CU_TRY(ctx->d_bstatus.reserve(nframes));
+  CU_TRY(ctx->d_brec.reserve(nframes));
+  CU_TRY(cudaMemcpy(ctx->d_bmax.p, max_n, (size_t) nframes * sizeof(long long), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(ctx->d_bstream.p, streams, (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(ctx->d_bpset.p, b.frame_set.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(ctx->d_brec.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemset(ctx->d_bstatus.p, 0, (size_t) nframes * sizeof(int)));
+  CU_TRY(cudaDeviceSynchronize());
+  b.on = true;
+  ctx->bound = std::move(b);
+  return PWPP_OK;
+}
+
+// One table launch, one unpack launch (capacities with points), then every run through launch_range_impl with grids sized for
+// its capacities. Never through launch_range: its own capture would nest inside a caller's.
+int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const auto t0 = std::chrono::steady_clock::now();
+  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
+  const pwpp_ctx::Bound& b = ctx->bound;
+  const int nf = b.nf;
+  // the host-side description launch_range_impl reads (direct calls between runs replace it)
+  ctx->last_nframes = nf;
+  ctx->runs = b.runs;
+  ctx->frame_set = b.frame_set;
+  ctx->chunk_off = b.cap_chunk_off;
+  ctx->pt_off = b.cap_pt_off;
+  k_bound_table<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                         ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p);
+  ++ctx->launches;
+  if (b.unpack_gx > 0) {
+    k_unpack_records<<<dim3((unsigned) b.unpack_gx, (unsigned) nf), REC_THREADS, 0, s>>>(ctx->d_brec.p, ctx->d_pt_off.p, ctx->d_in.p);
+    ++ctx->launches;
+  }
+  CU_TRY(cudaGetLastError());
+  for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
+    rc = launch_range_impl(ctx, b.runs[r], b.runs[r + 1] - b.runs[r], ctx->d_in.p, b.has_intensity, s, false, b.run_chunks[r]);
+    if (rc) return rc;
+  }
+  make_bound_last(ctx, s);
+  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
+  return PWPP_OK;
+}
+
+int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int64_t** d_offsets, const int32_t** d_num_ground,
+                            const int32_t** d_status) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  make_bound_last(ctx, ctx->last_stream ? ctx->last_stream : ctx->stream);
+  if (d_indices) *d_indices = ctx->d_out_idx.p;
+  if (d_offsets) *d_offsets = reinterpret_cast<const int64_t*>(ctx->d_pt_off.p);
+  if (d_num_ground) *d_num_ground = ctx->d_counts.p;
+  if (d_status) *d_status = ctx->d_bstatus.p;
+  return PWPP_OK;
+}
+
+int pwpp_unbind_call(pwpp_ctx* ctx) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound");
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
+  ctx->bound = pwpp_ctx::Bound();
+  return PWPP_OK;
+}
+
 // Record results of the last call: the first request gathers every frame's records into d_rec_out on the call's stream (one
 // launch, none when the call had no points), and no later request of the same call gathers again. The host blocks only where
 // a buffer is first reserved or grows, and on the previous request's offset-table upload (include/pwpp.h).
 static int gather_records(pwpp_ctx* ctx) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (ctx->last_nframes <= 0) return fail(PWPP_ERR_INVALID_ARG, "no estimate call yet");
+  if (ctx->last_bound)
+    return fail(PWPP_ERR_INVALID_ARG, "record results are not available for a bound call (pwpp_run_bound_call): their gather needs host offsets");
   if (ctx->last_recs.empty()) return fail(PWPP_ERR_INVALID_ARG, "the last estimate call did not take records (pwpp_estimate_host_records / pwpp_estimate_device_records)");
   if (ctx->rec_gathered) return PWPP_OK;
   int rc = bind_device(ctx);
@@ -1546,6 +1765,7 @@ int pwpp_device_results(pwpp_ctx* ctx, const int32_t** d_indices, const int32_t*
 int pwpp_set_output_order(pwpp_ctx* ctx, int order) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (order != PWPP_ORDER_BIN && order != PWPP_ORDER_REFERENCE) return fail(PWPP_ERR_INVALID_ARG, "order must be PWPP_ORDER_BIN or PWPP_ORDER_REFERENCE");
+  if (ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "the output order cannot change while a call is bound (it keeps the order it was bound with)");
   if (order != ctx->order_mode) ++g_alloc_gen;   // captured graphs were recorded with the other launch sequence
   ctx->order_mode = order;
   return PWPP_OK;
@@ -1608,6 +1828,8 @@ int pwpp_copy_bin_results(pwpp_ctx* ctx, int f, pwpp_bin_result* dst) {
 }
 int pwpp_copy_bin_ids(pwpp_ctx* ctx, int f, uint16_t* dst) {
   int rc = check_frame(ctx, f);
+  if (rc) return rc;
+  rc = fetch_offsets(ctx);
   if (rc) return rc;
   rc = bind_device(ctx);
   if (rc) return rc;

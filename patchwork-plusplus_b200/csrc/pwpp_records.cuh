@@ -133,6 +133,72 @@ inline RecordFrame record_frame(const pwpp_point_layout& L, const void* src) {
   return r;
 }
 
+// ---- bound calls (pwpp_bind_call / pwpp_run_bound_call): the frame tables from sizes that live on the device ---------------
+//
+// k_bound_table is one CTA. Thread t owns a contiguous slice of ceil(nf / BT_THREADS) frames: it accepts every count of its
+// slice (0 <= counts[f] <= max_n[f]; any other count makes an empty frame and sets status[f]), sums the accepted sizes and
+// their chunks, a warp-shuffle scan and a scan of the warp totals give every slice its start, and a second pass writes the
+// slice's entries: pt_off (int64 exclusive scan of the accepted counts, nf + 1 entries), chunk_off (scan of ceil(n / CHUNK_PTS),
+// nf + 1), status, and the bound call's own stream and set tables copied into the call tables, which direct calls between two
+// runs overwrite. The bind checked that the chunks of the capacities fit an int, so the accepted ones do too.
+constexpr int BT_THREADS = 1024;
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
+                                                            const int* __restrict__ b_stream, const int* __restrict__ b_pset,
+                                                            long long* __restrict__ pt_off, int* __restrict__ chunk_off, int* __restrict__ stream,
+                                                            int* __restrict__ pset, int* __restrict__ status) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int per = (nf + BT_THREADS - 1) / BT_THREADS;
+  const int f0 = tid * per < nf ? tid * per : nf;
+  const int f1 = f0 + per < nf ? f0 + per : nf;
+  long long own_pts = 0;
+  int own_chk = 0;
+  for (int f = f0; f < f1; ++f) {
+    const long long c = counts[f];
+    const long long n = (c >= 0 && c <= max_n[f]) ? c : 0;
+    own_pts += n;
+    own_chk += (int) ((n + CHUNK_PTS - 1) / CHUNK_PTS);
+  }
+  long long pts = own_pts;   // inclusive scan over the warp's slices
+  int chk = own_chk;
+  for (int d = 1; d < 32; d <<= 1) {
+    const long long p = __shfl_up_sync(0xffffffffu, pts, d);
+    const int q = __shfl_up_sync(0xffffffffu, chk, d);
+    if (lane >= d) { pts += p; chk += q; }
+  }
+  if (lane == 31) { s_pts[warp] = pts; s_chk[warp] = chk; }
+  __syncthreads();
+  if (warp == 0) {   // inclusive scan of the warp totals
+    long long wp = s_pts[lane];
+    int wc = s_chk[lane];
+    for (int d = 1; d < 32; d <<= 1) {
+      const long long p = __shfl_up_sync(0xffffffffu, wp, d);
+      const int q = __shfl_up_sync(0xffffffffu, wc, d);
+      if (lane >= d) { wp += p; wc += q; }
+    }
+    s_pts[lane] = wp;
+    s_chk[lane] = wc;
+  }
+  __syncthreads();
+  long long p = (warp > 0 ? s_pts[warp - 1] : 0) + pts - own_pts;   // start of the slice
+  int q = (warp > 0 ? s_chk[warp - 1] : 0) + chk - own_chk;
+  for (int f = f0; f < f1; ++f) {
+    const long long c = counts[f];
+    const bool ok = c >= 0 && c <= max_n[f];
+    const long long n = ok ? c : 0;
+    pt_off[f] = p;
+    chunk_off[f] = q;
+    status[f] = ok ? 0 : PWPP_COUNT_OUT_OF_RANGE;
+    stream[f] = b_stream[f];
+    pset[f] = b_pset[f];
+    p += n;
+    q += (int) ((n + CHUNK_PTS - 1) / CHUNK_PTS);
+  }
+  if (tid == BT_THREADS - 1) { pt_off[nf] = p; chunk_off[nf] = q; }   // the last slice ends at the totals
+}
+
 // grid.x of a launch over frames with these sizes and steps
 inline long long rec_grid_x(const long long* pt_off, const RecordFrame* recs, int nf) {
   long long gx = 0;

@@ -74,6 +74,10 @@ def load_library():
     lib.pwpp_set_output_order.argtypes = [vp, i32]; lib.pwpp_set_output_order.restype = i32
     lib.pwpp_host_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_host_results.restype = i32
     lib.pwpp_bind_host_to_device.argtypes = [i32]; lib.pwpp_bind_host_to_device.restype = i32
+    lib.pwpp_bind_call.argtypes = [vp, i32, vp, vp, vp, vp, vp]; lib.pwpp_bind_call.restype = i32
+    lib.pwpp_run_bound_call.argtypes = [vp, vp]; lib.pwpp_run_bound_call.restype = i32
+    lib.pwpp_bound_call_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_bound_call_results.restype = i32
+    lib.pwpp_unbind_call.argtypes = [vp]; lib.pwpp_unbind_call.restype = i32
     _lib = lib
     return lib
 
@@ -155,6 +159,7 @@ class Engine:
         self._n = []
         self._streams = []   # stream of every frame of the last call
         self._rec_dtypes = []   # record dtype of every frame of the last records call (uint8 rows of point_step for (buffer, layout) frames)
+        self._bound = None      # (frames, counts, streams, sum of max_n) of the bound call
 
     def close(self):
         if getattr(self, "_h", None):
@@ -267,6 +272,68 @@ class Engine:
         self._records_call(self.lib.pwpp_estimate_device_records, len(ptrs), streams, [int(p) for p in ptrs], ns, layouts, C.c_void_p(stream),
                            dtypes=dtypes)
 
+    # ---- bound call: frame sizes read on the GPU, capturable into a CUDA graph ----
+    def bind_call(self, frames, max_n, layouts, counts, streams=None):
+        """Binds a call whose frame sizes live on the device (pwpp_bind_call). Frame f is up to max_n[f] records of layouts[f] at
+        `frames[f]` (a device address or a CUDA tensor, any alignment), its size counts[f] of `counts`, an int64 CUDA tensor of
+        nframes entries read by the GPU at every run. `streams` as for estimate_host (None: frame f on stream f). The tensors are
+        kept alive while the call is bound; their contents may change between runs."""
+        import torch
+        nf = len(frames)
+        if not (isinstance(counts, torch.Tensor) and counts.is_cuda and counts.dtype == torch.int64 and counts.is_contiguous()
+                and counts.numel() == nf):
+            raise PwppError(f"counts must be a contiguous int64 CUDA tensor of {nf} entries")
+        ids = np.arange(nf, dtype=np.int32) if streams is None else self._stream_table(streams, nf)
+        ptrs = [int(fr.data_ptr()) if isinstance(fr, torch.Tensor) else int(fr) for fr in frames]
+        p = (C.c_void_p * max(nf, 1))(*ptrs)
+        n = (C.c_int64 * max(nf, 1))(*[int(k) for k in max_n])
+        lays = (PwppPointLayout * max(nf, 1))(*layouts)
+        _check(self.lib.pwpp_bind_call(self._h, nf, ids.ctypes.data, p, n, lays, C.c_void_p(counts.data_ptr())))
+        self._bound = (list(frames), counts, ids.tolist(), sum(int(k) for k in max_n))
+
+    def run_bound_call(self, stream: int = 0):
+        """Enqueues the bound call on CUDA stream `stream` (0: the ctx's own stream; inside torch.cuda.graph pass
+        torch.cuda.current_stream().cuda_stream). No host synchronisation: it may be captured and replayed."""
+        _check(self.lib.pwpp_run_bound_call(self._h, C.c_void_p(stream)))
+        self._use_bound()
+
+    def bound_call_results(self):
+        """Torch views of the bound call's device results (pwpp_bound_call_results): (indices int32[sum(max_n)], offsets
+        int64[nframes + 1], num_ground int32[nframes], status int32[nframes]). Frame f's lists start at offsets[f]: ground,
+        then non-ground. Fixed addresses while the call is bound. Also makes the bound call the last call of the host getters."""
+        import torch
+        a, b, c, d = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        _check(self.lib.pwpp_bound_call_results(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
+        self._use_bound()
+        frames, _, _, cap = self._bound
+        nf = len(frames)
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr, n, typestr):
+                self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 3, "strides": None}
+        idx = torch.as_tensor(_View(a.value, cap, "<i4"), device="cuda") if cap > 0 else torch.empty(0, dtype=torch.int32, device="cuda")
+        return (idx, torch.as_tensor(_View(b.value, nf + 1, "<i8"), device="cuda"), torch.as_tensor(_View(c.value, nf, "<i4"), device="cuda"),
+                torch.as_tensor(_View(d.value, nf, "<i4"), device="cuda"))
+
+    def unbind_call(self):
+        _check(self.lib.pwpp_unbind_call(self._h))
+        self._bound = None
+
+    def _use_bound(self):
+        """The host getters now serve the bound call: its frame sizes are fetched from the device when first needed."""
+        self._n = None
+        self._streams = list(self._bound[2])
+        self._rec_dtypes = []
+
+    def _sizes(self):
+        """Point count of every frame of the last call (after a bound call: from its device offsets, one device->host copy)."""
+        if self._n is None:
+            a, b, c = C.c_void_p(), C.c_void_p(), C.c_void_p()
+            _check(self.lib.pwpp_host_results(self._h, C.byref(a), C.byref(b), C.byref(c)))
+            nf = len(self._streams)
+            self._n = np.diff(np.ctypeslib.as_array((C.c_int64 * (nf + 1)).from_address(c.value))).tolist()
+        return self._n
+
     def synchronize(self):
         _check(self.lib.pwpp_synchronize(self._h))
 
@@ -368,8 +435,9 @@ class Engine:
         return arr
 
     def bin_ids(self, f=0):
-        out = np.empty(self._n[f], dtype=np.uint16)
-        if self._n[f] > 0:
+        n = self._sizes()[f]
+        out = np.empty(n, dtype=np.uint16)
+        if n > 0:
             _check(self.lib.pwpp_copy_bin_ids(self._h, f, out.ctypes.data))
         return out
 
@@ -400,7 +468,7 @@ class Engine:
         list. Valid until the next estimate call; the caller synchronizes with its stream (or Engine.synchronize())."""
         import torch
         d_idx, d_ng = self.device_results()
-        total, nf = int(sum(self._n)), len(self._n)
+        total, nf = int(sum(self._sizes())), len(self._sizes())
 
         class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
             def __init__(self, ptr, n):
@@ -415,7 +483,7 @@ class Engine:
         follows up to off[f + 1] (minus dropped points). Valid until the next estimate call."""
         a, b, c = C.c_void_p(), C.c_void_p(), C.c_void_p()
         _check(self.lib.pwpp_host_results(self._h, C.byref(a), C.byref(b), C.byref(c)))
-        total, nf = int(sum(self._n)), len(self._n)
+        total, nf = int(sum(self._sizes())), len(self._sizes())
         idx = np.ctypeslib.as_array((C.c_int32 * max(total, 1)).from_address(a.value))[:total]
         ng = np.ctypeslib.as_array((C.c_int32 * nf).from_address(b.value))
         off = np.ctypeslib.as_array((C.c_int64 * (nf + 1)).from_address(c.value))
