@@ -302,17 +302,47 @@ int pwpp_copy_nonground_records(pwpp_ctx* ctx, int f, void* dst);    /* num_nong
  *   - Shared state and results. Direct calls and runs of the bound call use the same stream state and the same result
  *     buffers; each one's results are valid until the next call or replay. The caller orders replays against direct calls
  *     (same stream, or its own events): the ctx cannot see a replay, and a capture cannot wait on an event recorded outside it.
- *   - pwpp_launch_count rises, per pwpp_run_bound_call, by one table launch, one unpack launch when any max_n > 0, and the
- *     usual launch sequence of each run (grids sized for the capacities).
- *   - The record results (pwpp_*_record_results, pwpp_copy_*_records) refuse a bound call with a message: their gather
- *     needs host offsets. */
+ *   - pwpp_launch_count rises, per pwpp_run_bound_call, by one table launch, one unpack launch when any max_n > 0, the
+ *     usual launch sequence of each run (grids sized for the capacities), and, once record results are enabled
+ *     (pwpp_bind_record_results), one gather launch, also when every max_n is 0.
+ *   - The record results of direct calls (pwpp_*_record_results, pwpp_copy_*_records) refuse a bound call with a message:
+ *     their gather needs host offsets. A bound call has record results of its own (below).
+ *
+ * Record results of the bound call: its ground and non-ground clouds as records of each frame's own layout (every field the
+ * sensor sent, byte for byte), gathered on the GPU at fixed addresses, for consumers that slice them without knowing any count
+ * on the host (a CUDA graph, a static-shape torch pipeline, a publisher of device buffers).
+ *
+ * pwpp_bind_record_results: enables them for the bound call. parts is PWPP_PART_GROUND, PWPP_PART_NONGROUND or both (3). Host
+ * work like pwpp_bind_call (it reserves the buffers, then synchronizes), so it is not capturable; graphs captured before it do
+ * not gather. From then on every pwpp_run_bound_call ends with one gather launch on its stream, after the last run's output
+ * kernel, with no host work. PWPP_ERR_INVALID_ARG when no call is bound, for parts outside {1, 2, 3}, and when record results
+ * are already enabled (one setting per bind: pwpp_unbind_call releases them, and a later bind starts with them off).
+ *
+ * Layout: one device buffer per enabled part. Frame f owns bytes [off[f], off[f + 1]) of each, off[f + 1] = off[f] +
+ * align16(max_n[f] * point_step_f) (the direct call's offsets with n = max_n; the same for both buffers). Every run writes, for
+ * every frame, num_ground(f) records at the start of the frame's ground region and num_nonground(f) records at the start of its
+ * non-ground region, record k = input record k of that list in the order the call was bound with (PWPP_ORDER_BIN or
+ * PWPP_ORDER_REFERENCE), and d_counts[2f] = ground, d_counts[2f + 1] = non-ground (int32), both counts whichever parts are
+ * enabled. A frame whose count was out of range ran as empty: its counts are 0 and its regions are not written. Bytes of a
+ * region past its count are never written. Memory: sum over frames of align16(max_n[f] * point_step_f) bytes per enabled part,
+ * plus 8 (nframes + 1) + 8 nframes bytes. The buffers are not work buffers: reserving them does not interact with the freeze.
+ *
+ * pwpp_bound_record_results: host-only. The fixed device pointers of the two buffers (NULL for a part that is not enabled), the
+ * host offsets off (nframes + 1) and the device counts int32[2 nframes]. PWPP_ERR_INVALID_ARG when no call is bound or record
+ * results are not enabled. Direct records calls between runs keep their own record results and never touch these buffers. */
 #define PWPP_COUNT_OUT_OF_RANGE 1   /* d_status[f]: d_counts[f] < 0 or > max_n[f]; the frame was run as an empty frame */
 int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
                    const pwpp_point_layout* layouts, const int64_t* d_counts);
 int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream);
 int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int64_t** d_offsets, const int32_t** d_num_ground,
                             const int32_t** d_status);
-/* Releases the bound call (PWPP_ERR_INVALID_ARG when none is bound). Its results stay readable until the next call. */
+#define PWPP_PART_GROUND 1
+#define PWPP_PART_NONGROUND 2
+int pwpp_bind_record_results(pwpp_ctx* ctx, int parts /* PWPP_PART_* bits: 1, 2 or 3 */);
+int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void** d_nonground, const int64_t** h_offsets,
+                              const int32_t** d_counts);
+/* Releases the bound call and its record results (PWPP_ERR_INVALID_ARG when none is bound). Its index results stay readable
+ * until the next call. */
 int pwpp_unbind_call(pwpp_ctx* ctx);
 
 /* cudaDeviceSynchronize() on the ctx's device: what a binding calls before handing device memory produced on an unknown

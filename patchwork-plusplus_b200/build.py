@@ -98,6 +98,12 @@ def build_examples(force=False):
     if force or _newer(out6, [src6] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out6, src6])
+    # the record gather of a bound call's record results, the same way (GPU cases of tests/test_records_parts_backends.py)
+    src8 = os.path.join(REPO, "tests", "gpu_records_parts_probe.cu")
+    out8 = os.path.join(LIB, "libpwpp_records_parts_probe.so")
+    if force or _newer(out8, [src8] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out8, src8])
     return out
 
 

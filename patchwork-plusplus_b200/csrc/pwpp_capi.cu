@@ -215,11 +215,18 @@ struct pwpp_ctx {
     long long unpack_gx = 0;                // grid.x of the unpack, from the capacities
     std::vector<int> runs, frame_set, run_chunks, cap_chunk_off;   // run_chunks[r]: the run's largest ceil(max_n / CHUNK_PTS)
     std::vector<long long> cap_pt_off;      // the capacity layout: sizes grids and picks the dense front end only
+    int rec_parts = 0;                      // record results (pwpp_bind_record_results): PWPP_PART_* bits, 0 = off
+    long long rec_gx = 0;                   // grid.x of k_gather_record_parts, from the capacities
+    std::vector<RecordFrame> recs;          // its record table (host copy of d_brec)
+    std::vector<long long> rec_part_off;    // [F+1] byte offsets of every frame's region in each part buffer
   } bound;
   DevBuf<long long, false> d_bmax;        // [F] max_n
   DevBuf<int, false> d_bstream, d_bpset;  // [F] the bound call's stream and set tables
   DevBuf<int, false> d_bstatus;           // [F] PWPP_COUNT_OUT_OF_RANGE or 0
   DevBuf<RecordFrame, false> d_brec;      // [F] its record table
+  DevBuf<unsigned char, false> d_bground, d_bnonground;   // its record results, one buffer per part (region f at rec_part_off[f])
+  DevBuf<long long, false> d_bpart_off;   // [F+1] rec_part_off
+  DevBuf<int, false> d_rec_counts;        // [F][2]: ground, non-ground records of every frame of the last run
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
   struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
@@ -963,6 +970,7 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   ctx->d_raw.release(); ctx->d_rec.release(); ctx->h_raw.release(); for (int i = 0; i < 2; ++i) ctx->h_rec_buf[i].release();
   ctx->d_rec_out.release(); ctx->d_rec_off.release(); ctx->h_rec_off.release(); ctx->h_rec_out.release();
   ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
+  ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
   if (ctx->ev_rec_off) cudaEventDestroy(ctx->ev_rec_off);
   ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
   ctx->h_out_idx.release(); ctx->h_counts.release();
@@ -1410,6 +1418,7 @@ int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const voi
     b.frame_set.push_back(ctx->stream_set[streams[f]]);
   }
   b.unpack_gx = b.cap_pt_off[nframes] > 0 ? rec_grid_x(b.cap_pt_off.data(), recs.data(), nframes) : 0;
+  b.recs = recs;
   split_runs(ctx, nframes, streams);
   b.runs = ctx->runs;
   for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
@@ -1471,6 +1480,14 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     rc = launch_range_impl(ctx, b.runs[r], b.runs[r + 1] - b.runs[r], ctx->d_in.p, b.has_intensity, s, false, b.run_chunks[r]);
     if (rc) return rc;
   }
+  if (b.rec_parts) {   // the record results: both parts' lists are where the runs' k_emit left them
+    const int first = b.rec_parts == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.rec_parts == 3 ? 2 : 1;
+    k_gather_record_parts<<<dim3((unsigned) b.rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
+        ctx->d_brec.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, ctx->d_bpart_off.p, first, ctx->d_bground.p, ctx->d_bnonground.p,
+        ctx->d_rec_counts.p);
+    ++ctx->launches;
+    CU_TRY(cudaGetLastError());
+  }
   make_bound_last(ctx, s);
   ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
   return PWPP_OK;
@@ -1494,7 +1511,46 @@ int pwpp_unbind_call(pwpp_ctx* ctx) {
   int rc = bind_device(ctx);
   if (rc) return rc;
   ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
+  ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
   ctx->bound = pwpp_ctx::Bound();
+  return PWPP_OK;
+}
+
+int pwpp_bind_record_results(pwpp_ctx* ctx, int parts) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
+  if (b.rec_parts) return fail(PWPP_ERR_INVALID_ARG, "record results are already enabled for the bound call");
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const int nf = b.nf;
+  std::vector<long long> off(nf + 1);   // the direct call's region layout with n = max_n
+  rec_out_offsets(b.cap_pt_off.data(), b.recs.data(), nf, off.data());
+  const size_t bytes = (size_t) std::max<long long>(off[nf], 16);
+  if (parts & PWPP_PART_GROUND) CU_TRY(ctx->d_bground.reserve(bytes));
+  if (parts & PWPP_PART_NONGROUND) CU_TRY(ctx->d_bnonground.reserve(bytes));
+  CU_TRY(ctx->d_bpart_off.reserve(nf + 1));
+  CU_TRY(ctx->d_rec_counts.reserve(2 * (size_t) nf));
+  CU_TRY(cudaMemcpy(ctx->d_bpart_off.p, off.data(), (size_t) (nf + 1) * sizeof(long long), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemset(ctx->d_rec_counts.p, 0, 2 * (size_t) nf * sizeof(int)));
+  CU_TRY(cudaDeviceSynchronize());
+  b.rec_part_off = std::move(off);
+  b.rec_gx = rec_parts_grid_x(b.cap_pt_off.data(), b.recs.data(), nf);
+  b.rec_parts = parts;
+  return PWPP_OK;
+}
+
+int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void** d_nonground, const int64_t** h_offsets,
+                              const int32_t** d_counts) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  const pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (!b.rec_parts) return fail(PWPP_ERR_INVALID_ARG, "record results are not enabled for the bound call (pwpp_bind_record_results)");
+  if (d_ground) *d_ground = (b.rec_parts & PWPP_PART_GROUND) ? ctx->d_bground.p : nullptr;
+  if (d_nonground) *d_nonground = (b.rec_parts & PWPP_PART_NONGROUND) ? ctx->d_bnonground.p : nullptr;
+  if (h_offsets) *h_offsets = reinterpret_cast<const int64_t*>(b.rec_part_off.data());
+  if (d_counts) *d_counts = ctx->d_rec_counts.p;
   return PWPP_OK;
 }
 
@@ -1505,7 +1561,7 @@ static int gather_records(pwpp_ctx* ctx) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (ctx->last_nframes <= 0) return fail(PWPP_ERR_INVALID_ARG, "no estimate call yet");
   if (ctx->last_bound)
-    return fail(PWPP_ERR_INVALID_ARG, "record results are not available for a bound call (pwpp_run_bound_call): their gather needs host offsets");
+    return fail(PWPP_ERR_INVALID_ARG, "record results are not available for a bound call (pwpp_run_bound_call): their gather needs host offsets (pwpp_bind_record_results gives a bound call its own)");
   if (ctx->last_recs.empty()) return fail(PWPP_ERR_INVALID_ARG, "the last estimate call did not take records (pwpp_estimate_host_records / pwpp_estimate_device_records)");
   if (ctx->rec_gathered) return PWPP_OK;
   int rc = bind_device(ctx);

@@ -254,28 +254,13 @@ __device__ __forceinline__ unsigned rec_src4(const unsigned char* p, const unsig
   return rec_bytes4(p, hi);
 }
 
-// frame f = blockIdx.y: output records [k0, k0 + tile) of its region. recs / pt_off / rec_off / nd are the call's tables (the
-// unpack's record table, point offsets, byte offsets of the output regions, dropped counts), idx the index lists.
-__global__ void __launch_bounds__(REC_THREADS, 4) k_gather_records(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
-                                                                 const long long* __restrict__ rec_off, const int* __restrict__ nd,
-                                                                 const int* __restrict__ idx,
-                                                                 unsigned char* __restrict__ dst) {
-  __shared__ __align__(16) unsigned s_w[REC_SMEM_WORDS];
-  __shared__ int s_idx[REC_MAX_TILE_PTS];
-  const int f = blockIdx.y, tid = threadIdx.x;
-  const long long p0 = pt_off[f];
-  const long long n = pt_off[f + 1] - p0;
-  const long long m = n - nd[f];                       // ground + non-ground records of the frame
-  const int step = recs[f].step;
-  const int tp = rec_tile_pts(step);
-  const long long k0 = (long long) blockIdx.x * tp;
-  if (k0 >= m) return;
-  const int cnt = (int) (m - k0 < tp ? m - k0 : tp);
-  const unsigned char* lo = recs[f].src;
-  const unsigned char* hi = lo + n * step;
-  for (int i = tid; i < cnt; i += REC_THREADS) s_idx[i] = idx[p0 + k0 + i];
-  unsigned char* a = dst + rec_off[f] + k0 * step;          // the tile's bytes [a, b) of dst
-  unsigned char* b = a + (size_t) cnt * step;
+// One tile of a record gather, run by every thread of the CTA: output record i (0 <= i < cnt <= rec_tile_pts(step)) = source
+// record idx[i0 + i] of the frame [lo, hi), written to a + i * step. s_w and s_idx are the caller's shared arrays.
+__device__ __forceinline__ void rec_gather_tile(const unsigned char* lo, const unsigned char* hi, int step, const int* __restrict__ idx, long long i0,
+                                                int cnt, unsigned char* a, unsigned* s_w, int* s_idx) {
+  const int tid = threadIdx.x;
+  for (int i = tid; i < cnt; i += REC_THREADS) s_idx[i] = idx[i0 + i];
+  unsigned char* b = a + (size_t) cnt * step;               // the tile's bytes [a, b) of dst
   unsigned char* a_floor = (unsigned char*) ((uintptr_t) a & ~(uintptr_t) 15);   // shared word 0 stands for this address
   const int r0 = (int) (a - a_floor), r1 = r0 + cnt * step;   // the tile's bytes in shared memory
   __syncthreads();
@@ -364,10 +349,69 @@ __global__ void __launch_bounds__(REC_THREADS, 4) k_gather_records(const RecordF
   }
 }
 
+// frame f = blockIdx.y: output records [k0, k0 + tile) of its region. recs / pt_off / rec_off / nd are the call's tables (the
+// unpack's record table, point offsets, byte offsets of the output regions, dropped counts), idx the index lists.
+__global__ void __launch_bounds__(REC_THREADS, 4) k_gather_records(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
+                                                                 const long long* __restrict__ rec_off, const int* __restrict__ nd,
+                                                                 const int* __restrict__ idx,
+                                                                 unsigned char* __restrict__ dst) {
+  __shared__ __align__(16) unsigned s_w[REC_SMEM_WORDS];
+  __shared__ int s_idx[REC_MAX_TILE_PTS];
+  const int f = blockIdx.y;
+  const long long p0 = pt_off[f];
+  const long long n = pt_off[f + 1] - p0;
+  const long long m = n - nd[f];                       // ground + non-ground records of the frame
+  const int step = recs[f].step;
+  const int tp = rec_tile_pts(step);
+  const long long k0 = (long long) blockIdx.x * tp;
+  if (k0 >= m) return;
+  const int cnt = (int) (m - k0 < tp ? m - k0 : tp);
+  const unsigned char* lo = recs[f].src;
+  rec_gather_tile(lo, lo + n * step, step, idx, p0 + k0, cnt, dst + rec_off[f] + k0 * step, s_w, s_idx);
+}
+
+// ---- record results of a bound call (pwpp_bind_record_results): one buffer per part, regions fixed by the capacities -------
+//
+// k_gather_record_parts writes part z = first + blockIdx.z (0 ground, 1 non-ground) of frame f = blockIdx.y: output record k of
+// the part's list = input record idx[start + k], to dst_z + part_off[f] + k * step. The list is found on the device: the ground
+// list starts at pt_off[f] and holds counts[f] records, the non-ground list follows it and holds n - counts[f] - counts[2 nf + f]
+// (counts: the call's count rows, num_ground, num_patches, num_dropped). The grid is sized from the capacities, so CTAs past the
+// list return at once; CTA (0, f, 0) writes both counts of the frame to part_cnt[2f], part_cnt[2f + 1], whichever parts run.
+// Frame f's tiles stay inside [part_off[f], part_off[f] + count * step) and read only [src, src + n * step).
+__global__ void __launch_bounds__(REC_THREADS, 4) k_gather_record_parts(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
+                                                                      const int* __restrict__ counts, int nf, const int* __restrict__ idx,
+                                                                      const long long* __restrict__ part_off, int first,
+                                                                      unsigned char* __restrict__ ground, unsigned char* __restrict__ nonground,
+                                                                      int* __restrict__ part_cnt) {
+  __shared__ __align__(16) unsigned s_w[REC_SMEM_WORDS];
+  __shared__ int s_idx[REC_MAX_TILE_PTS];
+  const int f = blockIdx.y, part = first + (int) blockIdx.z;
+  const long long p0 = pt_off[f];
+  const long long n = pt_off[f + 1] - p0;
+  const int ng = counts[f];
+  const long long nn = n - ng - counts[2 * nf + f];
+  if (blockIdx.x == 0 && blockIdx.z == 0 && threadIdx.x == 0) { part_cnt[2 * f] = ng; part_cnt[2 * f + 1] = (int) nn; }
+  const long long m = part ? nn : ng;
+  const int step = recs[f].step;
+  const int tp = rec_tile_pts(step);
+  const long long k0 = (long long) blockIdx.x * tp;
+  if (k0 >= m) return;
+  const int cnt = (int) (m - k0 < tp ? m - k0 : tp);
+  const unsigned char* lo = recs[f].src;
+  unsigned char* dst = part ? nonground : ground;
+  rec_gather_tile(lo, lo + n * step, step, idx, p0 + (part ? ng : 0) + k0, cnt, dst + part_off[f] + k0 * step, s_w, s_idx);
+}
+
 // Byte offsets of every frame's output region (16-byte aligned, room for all n[f] records): off[nf + 1].
 inline void rec_out_offsets(const long long* pt_off, const RecordFrame* recs, int nf, long long* off) {
   off[0] = 0;
   for (int f = 0; f < nf; ++f) off[f + 1] = off[f] + (((pt_off[f + 1] - pt_off[f]) * recs[f].step + 15) & ~15LL);
+}
+
+// grid.x of k_gather_record_parts over frames of these capacities: the tiles of the largest, at least 1 (the counts are written)
+inline long long rec_parts_grid_x(const long long* cap_off, const RecordFrame* recs, int nf) {
+  const long long gx = rec_grid_x(cap_off, recs, nf);
+  return gx > 0 ? gx : 1;
 }
 
 }  // namespace pwpp

@@ -78,6 +78,9 @@ def load_library():
     lib.pwpp_run_bound_call.argtypes = [vp, vp]; lib.pwpp_run_bound_call.restype = i32
     lib.pwpp_bound_call_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_bound_call_results.restype = i32
     lib.pwpp_unbind_call.argtypes = [vp]; lib.pwpp_unbind_call.restype = i32
+    lib.pwpp_bind_record_results.argtypes = [vp, i32]; lib.pwpp_bind_record_results.restype = i32
+    lib.pwpp_bound_record_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    lib.pwpp_bound_record_results.restype = i32
     _lib = lib
     return lib
 
@@ -314,6 +317,36 @@ class Engine:
         idx = torch.as_tensor(_View(a.value, cap, "<i4"), device="cuda") if cap > 0 else torch.empty(0, dtype=torch.int32, device="cuda")
         return (idx, torch.as_tensor(_View(b.value, nf + 1, "<i8"), device="cuda"), torch.as_tensor(_View(c.value, nf, "<i4"), device="cuda"),
                 torch.as_tensor(_View(d.value, nf, "<i4"), device="cuda"))
+
+    def bind_record_results(self, ground: bool = True, nonground: bool = True):
+        """Enables the bound call's record results (pwpp_bind_record_results): every later run_bound_call, and every graph captured
+        after this, also gathers the ground and / or non-ground records of every frame into fixed device buffers. Host work
+        that synchronizes: call it before a capture, not inside one."""
+        parts = (1 if ground else 0) | (2 if nonground else 0)
+        _check(self.lib.pwpp_bind_record_results(self._h, parts))
+
+    def bound_record_results(self):
+        """(ground, nonground, offsets, counts) of the bound call's record results (pwpp_bound_record_results): ground and
+        nonground are zero-copy uint8 CUDA tensors of offsets[-1] bytes (None for a part that is not enabled), offsets int64
+        numpy [nframes + 1] (frame f's region of each starts at offsets[f]), counts an int32 CUDA tensor view (nframes, 2) of
+        every frame's ground and non-ground record counts. Frame f's non-ground cloud after a run or replay is
+        nonground[offsets[f]: offsets[f] + counts[f, 1] * point_step]. Fixed addresses while the call is bound."""
+        import torch
+        a, b, c, d = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        _check(self.lib.pwpp_bound_record_results(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
+        nf = len(self._bound[0])
+        off = np.ctypeslib.as_array((C.c_int64 * (nf + 1)).from_address(c.value)).copy()
+        total = int(off[-1])
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr, shape, typestr):
+                self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (ptr, False), "version": 3, "strides": None}
+
+        def part(ptr):
+            if not ptr:
+                return None
+            return torch.as_tensor(_View(ptr, (total,), "|u1"), device="cuda") if total > 0 else torch.empty(0, dtype=torch.uint8, device="cuda")
+        return part(a.value), part(b.value), off, torch.as_tensor(_View(d.value, (nf, 2), "<i4"), device="cuda")
 
     def unbind_call(self):
         _check(self.lib.pwpp_unbind_call(self._h))
