@@ -333,6 +333,41 @@ int pwpp_copy_nonground_records(pwpp_ctx* ctx, int f, void* dst);    /* num_nong
 #define PWPP_COUNT_OUT_OF_RANGE 1   /* d_status[f]: d_counts[f] < 0 or > max_n[f]; the frame was run as an empty frame */
 int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
                    const pwpp_point_layout* layouts, const int64_t* d_counts);
+
+/* Per-frame actions of a bound call, for sensors that do not tick together: a frame can be left out of a run, or its stream
+ * reset first, decided on the GPU at every run or replay. A count of 0 is not the same as leaving a frame out: an empty frame
+ * still runs the threshold update, which moves the state of a stream whose histories are full.
+ *
+ * pwpp_bind_call_actions: pwpp_bind_call plus d_actions, a device int32 array of nframes actions that the GPU reads at every
+ * run or replay, like d_counts. d_actions == NULL is exactly pwpp_bind_call. The actions are a bind argument because skipping
+ * needs scratch state slots (below), and reserving them later would move the state buffers under a graph already captured.
+ *   - PWPP_FRAME_RUN: the frame runs as with pwpp_bind_call.
+ *   - PWPP_FRAME_SKIP: the frame is absent from this run. It runs as an empty frame whose count is neither read nor
+ *     validated; its stream's complete state (the export blob: histories and the carried plane included) stays bit for bit
+ *     what it was. Its results by position are those of an empty frame (an empty list span in the offsets, num_ground 0, no
+ *     patches), its record-result counts are 0 and its record regions are not written. d_status[f] = PWPP_FRAME_SKIPPED.
+ *   - PWPP_FRAME_RESET: the stream is restored to its set's constructor state, as by pwpp_reset_stream, immediately before
+ *     this frame (after the stream's earlier frames of the bound call have run), then the frame runs as RUN would. An
+ *     out-of-range count still gives PWPP_COUNT_OUT_OF_RANGE and an empty frame, with the reset applied; RESET with count 0
+ *     is "reset only": the state equals a freshly reset stream's, bit for bit.
+ *   - Any other value: the frame is skipped and d_status[f] = PWPP_ACTION_INVALID (a replay cannot return an error).
+ *   - Each run reads every action once, in its first kernel, into a copy the ctx owns; the later kernels of the run read the
+ *     copy, so rewriting d_actions during a run never splits one frame's action between kernels.
+ *   - pwpp_launch_count rises, compared with the same call bound without actions, by one reset launch for each run that holds
+ *     a frame whose stream also has a frame in an earlier run. A bound call without repeated streams has no extra launch.
+ *   - Scratch slots: a skipped frame is redirected to a scratch state slot, so the kernels see an ordinary empty frame and the
+ *     real stream is never written. The bind grows the state and history buffers by L slots, L the longest run of the call (at
+ *     most num_streams), sizeof(state) + 64 * history capacity bytes each (about 82 KB with the default parameters); the
+ *     streams' states are copied across, a failed allocation leaves them as they were, and growing them makes graphs captured
+ *     earlier by the ctx's own small calls capture again. The slots stay reserved after pwpp_unbind_call.
+ *   - The freeze, pwpp_unbind_call and the record results behave as for pwpp_bind_call. */
+#define PWPP_FRAME_RUN 0        /* the frame runs as with pwpp_bind_call */
+#define PWPP_FRAME_SKIP 1       /* the frame is absent from this run */
+#define PWPP_FRAME_RESET 2      /* reset the stream to its set's constructor state, then run the frame */
+#define PWPP_FRAME_SKIPPED 2    /* d_status[f]: the frame's action was PWPP_FRAME_SKIP */
+#define PWPP_ACTION_INVALID 3   /* d_status[f]: the frame's action was not a PWPP_FRAME_* value; it was skipped */
+int pwpp_bind_call_actions(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
+                           const pwpp_point_layout* layouts, const int64_t* d_counts, const int32_t* d_actions);
 int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream);
 int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int64_t** d_offsets, const int32_t** d_num_ground,
                             const int32_t** d_status);

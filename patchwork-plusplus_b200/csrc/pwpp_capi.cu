@@ -67,6 +67,21 @@ struct DevBuf {
     if (e == cudaSuccess) cap = want;
     return e;
   }
+  // reserve that keeps the contents (synchronous); when the allocation fails the buffer stays as it was
+  cudaError_t grow_keep(size_t n) {
+    if (n <= cap) return cudaSuccess;
+    const size_t want = n + n / 8 + 64;
+    T* q = nullptr;
+    cudaError_t e = cudaMalloc(&q, want * sizeof(T));
+    if (e != cudaSuccess) return e;
+    if (p) e = cudaMemcpy(q, p, cap * sizeof(T), cudaMemcpyDeviceToDevice);
+    if (e != cudaSuccess) { cudaFree(q); return e; }
+    if (InGraphs) ++g_alloc_gen;
+    if (p) cudaFree(p);
+    p = q;
+    cap = want;
+    return cudaSuccess;
+  }
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 template <typename T>
@@ -219,7 +234,10 @@ struct pwpp_ctx {
     long long rec_gx = 0;                   // grid.x of k_gather_record_parts, from the capacities
     std::vector<RecordFrame> recs;          // its record table (host copy of d_brec)
     std::vector<long long> rec_part_off;    // [F+1] byte offsets of every frame's region in each part buffer
+    const int* d_actions = nullptr;         // the caller's device actions (pwpp_bind_call_actions), NULL: none
+    std::vector<char> reset_run;            // [runs] the run holds a frame whose stream ran in an earlier run: k_bound_reset
   } bound;
+  int scratch_slots = 0;                  // state / history slots after the streams' (pwpp_bind_call_actions), kept after unbind
   DevBuf<long long, false> d_bmax;        // [F] max_n
   DevBuf<int, false> d_bstream, d_bpset;  // [F] the bound call's stream and set tables
   DevBuf<int, false> d_bstatus;           // [F] PWPP_COUNT_OUT_OF_RANGE or 0
@@ -227,6 +245,8 @@ struct pwpp_ctx {
   DevBuf<unsigned char, false> d_bground, d_bnonground;   // its record results, one buffer per part (region f at rec_part_off[f])
   DevBuf<long long, false> d_bpart_off;   // [F+1] rec_part_off
   DevBuf<int, false> d_rec_counts;        // [F][2]: ground, non-ground records of every frame of the last run
+  DevBuf<int, false> d_bscratch, d_bdep;  // [F] with actions: scratch slot of every frame; its stream has a frame in an earlier run
+  DevBuf<int, false> d_bact;              // [F] the run's copy of the actions
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
   struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
@@ -971,6 +991,7 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   ctx->d_rec_out.release(); ctx->d_rec_off.release(); ctx->h_rec_off.release(); ctx->h_rec_out.release();
   ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
   ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
+  ctx->d_bscratch.release(); ctx->d_bdep.release(); ctx->d_bact.release();
   if (ctx->ev_rec_off) cudaEventDestroy(ctx->ev_rec_off);
   ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
   ctx->h_out_idx.release(); ctx->h_counts.release();
@@ -1395,6 +1416,13 @@ static void make_bound_last(pwpp_ctx* ctx, cudaStream_t s) {
 
 int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
                    const pwpp_point_layout* layouts, const int64_t* d_counts) {
+  return pwpp_bind_call_actions(ctx, nframes, streams, frames, max_n, layouts, d_counts, nullptr);
+}
+
+// With actions: frame f of run r gets scratch slot num_streams + (f - runs[r]) (distinct inside a run), and dep[f] says whether
+// its stream has a frame in an earlier run (then a RESET of f waits for that run: k_bound_reset before f's run).
+int pwpp_bind_call_actions(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
+                           const pwpp_point_layout* layouts, const int64_t* d_counts, const int32_t* d_actions) {
   int rc = check_records_call(ctx, nframes, streams, frames, max_n, layouts);
   if (rc) return rc;
   if (ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "a call is already bound (pwpp_unbind_call releases it)");
@@ -1426,6 +1454,25 @@ int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const voi
     for (int f = b.runs[r]; f < b.runs[r + 1]; ++f) m = std::max(m, b.cap_chunk_off[f + 1] - b.cap_chunk_off[f]);
     b.run_chunks.push_back(m);
   }
+  std::vector<int> scratch, dep;
+  int slots = 0;   // the longest run
+  if (d_actions) {
+    b.d_actions = d_actions;
+    scratch.resize(nframes);
+    dep.resize(nframes);
+    std::vector<int> first_run(ctx->num_streams, -1);
+    b.reset_run.assign(b.runs.size() - 1, 0);
+    for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
+      slots = std::max(slots, b.runs[r + 1] - b.runs[r]);
+      for (int f = b.runs[r]; f < b.runs[r + 1]; ++f) {
+        int& fr = first_run[streams[f]];
+        if (fr < 0) fr = (int) r;
+        scratch[f] = ctx->num_streams + (f - b.runs[r]);
+        dep[f] = fr < (int) r;
+        if (dep[f]) b.reset_run[r] = 1;
+      }
+    }
+  }
   rc = bind_device(ctx);
   if (rc) return rc;
   // the buffers may move: whatever the ctx enqueued before has finished with them, and the last call's results end here
@@ -1433,8 +1480,31 @@ int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const voi
   CU_TRY(cudaStreamSynchronize(ctx->stream));
   ctx->last_nframes = 0;
   ctx->last_bound = false;
+  if (slots > ctx->scratch_slots) {
+    // the streams' states and histories move with their contents; a failed allocation leaves them where they were
+    const size_t ns = (size_t) ctx->num_streams + slots;
+    CU_TRY(ctx->d_states.grow_keep(ns));
+    CU_TRY(ctx->d_hist.grow_keep(ns * 2 * 4 * ctx->hist_stride));
+    ctx->scratch_slots = slots;
+  }
+  if (slots > 0) {
+    // a scratch slot starts as a constructor state (empty histories): the empty frames redirected there keep it empty, so
+    // k_gle never reads a history sample of a scratch slot
+    StreamState s0;
+    CU_TRY(cudaMemcpy(&s0, ctx->d_states_init.p, sizeof(StreamState), cudaMemcpyDeviceToHost));
+    const std::vector<StreamState> fill(slots, s0);
+    CU_TRY(cudaMemcpy(ctx->d_states.p + ctx->num_streams, fill.data(), (size_t) slots * sizeof(StreamState), cudaMemcpyHostToDevice));
+  }
   rc = reserve_work(ctx, nframes, b.cap_pt_off[nframes], chunks, true, false);
   if (rc) return rc;
+  if (d_actions) {
+    CU_TRY(ctx->d_bscratch.reserve(nframes));
+    CU_TRY(ctx->d_bdep.reserve(nframes));
+    CU_TRY(ctx->d_bact.reserve(nframes));
+    CU_TRY(cudaMemcpy(ctx->d_bscratch.p, scratch.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemcpy(ctx->d_bdep.p, dep.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemset(ctx->d_bact.p, 0, (size_t) nframes * sizeof(int)));
+  }
   CU_TRY(ctx->d_bmax.reserve(nframes));
   CU_TRY(ctx->d_bstream.reserve(nframes));
   CU_TRY(ctx->d_bpset.reserve(nframes));
@@ -1468,8 +1538,14 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   ctx->frame_set = b.frame_set;
   ctx->chunk_off = b.cap_chunk_off;
   ctx->pt_off = b.cap_pt_off;
-  k_bound_table<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
-                                         ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p);
+  if (b.d_actions) {
+    const BoundActions A{b.d_actions, ctx->d_bact.p, ctx->d_bscratch.p, ctx->d_bdep.p, ctx->d_states_init.p, ctx->d_states.p};
+    k_bound_table_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                                   ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p, A);
+  } else {
+    k_bound_table<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                           ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p);
+  }
   ++ctx->launches;
   if (b.unpack_gx > 0) {
     k_unpack_records<<<dim3((unsigned) b.unpack_gx, (unsigned) nf), REC_THREADS, 0, s>>>(ctx->d_brec.p, ctx->d_pt_off.p, ctx->d_in.p);
@@ -1477,6 +1553,11 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   }
   CU_TRY(cudaGetLastError());
   for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
+    if (b.d_actions && b.reset_run[r]) {   // the RESET frames whose stream ran in an earlier run
+      k_bound_reset<<<1, BR_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], ctx->d_bact.p, ctx->d_bdep.p, ctx->d_bstream.p, ctx->d_states_init.p, ctx->d_states.p);
+      ++ctx->launches;
+      CU_TRY(cudaGetLastError());
+    }
     rc = launch_range_impl(ctx, b.runs[r], b.runs[r + 1] - b.runs[r], ctx->d_in.p, b.has_intensity, s, false, b.run_chunks[r]);
     if (rc) return rc;
   }
@@ -1512,6 +1593,7 @@ int pwpp_unbind_call(pwpp_ctx* ctx) {
   if (rc) return rc;
   ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
   ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
+  ctx->d_bscratch.release(); ctx->d_bdep.release(); ctx->d_bact.release();
   ctx->bound = pwpp_ctx::Bound();
   return PWPP_OK;
 }

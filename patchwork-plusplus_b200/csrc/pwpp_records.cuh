@@ -141,14 +141,40 @@ inline RecordFrame record_frame(const pwpp_point_layout& L, const void* src) {
 // slice's entries: pt_off (int64 exclusive scan of the accepted counts, nf + 1 entries), chunk_off (scan of ceil(n / CHUNK_PTS),
 // nf + 1), status, and the bound call's own stream and set tables copied into the call tables, which direct calls between two
 // runs overwrite. The bind checked that the chunks of the capacities fit an int, so the accepted ones do too.
+//
+// With per-frame actions (pwpp_bind_call_actions) the same kernel, k_bound_table_actions, also reads every frame's action once
+// (actions[f], the caller's device array) into the ctx's copy act[f], which every later kernel of the run reads. A frame that is
+// not PWPP_FRAME_RUN or PWPP_FRAME_RESET is skipped: its count is not read, it runs as an empty frame, status[f] is
+// PWPP_FRAME_SKIPPED (PWPP_ACTION_INVALID for an unknown value), and stream[f] is its scratch slot scratch[f], so k_gle writes
+// the empty frame's update there and the real stream is never touched. A RESET frame whose stream has no frame in an earlier
+// run (dep[f] == 0) gets its stream's constructor state here, before any run; the others are reset by k_bound_reset right
+// before their run.
 constexpr int BT_THREADS = 1024;
 
-__global__ void __launch_bounds__(BT_THREADS) k_bound_table(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
-                                                            const int* __restrict__ b_stream, const int* __restrict__ b_pset,
-                                                            long long* __restrict__ pt_off, int* __restrict__ chunk_off, int* __restrict__ stream,
-                                                            int* __restrict__ pset, int* __restrict__ status) {
-  __shared__ long long s_pts[BT_THREADS / 32];
-  __shared__ int s_chk[BT_THREADS / 32];
+struct BoundActions {
+  const int* actions;            // the caller's device actions [nf]
+  int* act;                      // the ctx's copy [nf]
+  const int* scratch;            // scratch slot of every frame [nf]
+  const int* dep;                // 1: the frame's stream has a frame in an earlier run [nf]
+  const StreamState* init;       // constructor state of every stream
+  StreamState* states;
+};
+
+// frame f's action from the caller's array, copied for the later kernels of the run (actions of a bound call without them: RUN)
+template <bool Actions>
+__device__ __forceinline__ int bt_action(const BoundActions& A, int f) {
+  if (!Actions) return PWPP_FRAME_RUN;
+  const int a = A.actions[f];
+  A.act[f] = a;
+  return a;
+}
+__device__ __forceinline__ bool bt_runs(int a) { return a == PWPP_FRAME_RUN || a == PWPP_FRAME_RESET; }
+
+template <bool Actions>
+__device__ __forceinline__ void bound_table_body(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
+                                                 const int* __restrict__ b_stream, const int* __restrict__ b_pset, long long* __restrict__ pt_off,
+                                                 int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
+                                                 int* __restrict__ status, const BoundActions& A, long long* s_pts, int* s_chk) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int per = (nf + BT_THREADS - 1) / BT_THREADS;
   const int f0 = tid * per < nf ? tid * per : nf;
@@ -156,8 +182,11 @@ __global__ void __launch_bounds__(BT_THREADS) k_bound_table(int nf, const long l
   long long own_pts = 0;
   int own_chk = 0;
   for (int f = f0; f < f1; ++f) {
-    const long long c = counts[f];
-    const long long n = (c >= 0 && c <= max_n[f]) ? c : 0;
+    long long n = 0;
+    if (bt_runs(bt_action<Actions>(A, f))) {
+      const long long c = counts[f];
+      n = (c >= 0 && c <= max_n[f]) ? c : 0;
+    }
     own_pts += n;
     own_chk += (int) ((n + CHUNK_PTS - 1) / CHUNK_PTS);
   }
@@ -185,6 +214,18 @@ __global__ void __launch_bounds__(BT_THREADS) k_bound_table(int nf, const long l
   long long p = (warp > 0 ? s_pts[warp - 1] : 0) + pts - own_pts;   // start of the slice
   int q = (warp > 0 ? s_chk[warp - 1] : 0) + chk - own_chk;
   for (int f = f0; f < f1; ++f) {
+    if (Actions) {
+      const int a = A.act[f];   // this thread's own copy from the first pass
+      if (!bt_runs(a)) {
+        pt_off[f] = p;
+        chunk_off[f] = q;
+        status[f] = a == PWPP_FRAME_SKIP ? PWPP_FRAME_SKIPPED : PWPP_ACTION_INVALID;
+        stream[f] = A.scratch[f];
+        pset[f] = b_pset[f];
+        continue;
+      }
+      if (a == PWPP_FRAME_RESET && !A.dep[f]) A.states[b_stream[f]] = A.init[b_stream[f]];
+    }
     const long long c = counts[f];
     const bool ok = c >= 0 && c <= max_n[f];
     const long long n = ok ? c : 0;
@@ -197,6 +238,37 @@ __global__ void __launch_bounds__(BT_THREADS) k_bound_table(int nf, const long l
     q += (int) ((n + CHUNK_PTS - 1) / CHUNK_PTS);
   }
   if (tid == BT_THREADS - 1) { pt_off[nf] = p; chunk_off[nf] = q; }   // the last slice ends at the totals
+}
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
+                                                            const int* __restrict__ b_stream, const int* __restrict__ b_pset,
+                                                            long long* __restrict__ pt_off, int* __restrict__ chunk_off, int* __restrict__ stream,
+                                                            int* __restrict__ pset, int* __restrict__ status) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<false>(nf, counts, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, BoundActions{}, s_pts, s_chk);
+}
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table_actions(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
+                                                                    const int* __restrict__ b_stream, const int* __restrict__ b_pset,
+                                                                    long long* __restrict__ pt_off, int* __restrict__ chunk_off, int* __restrict__ stream,
+                                                                    int* __restrict__ pset, int* __restrict__ status, const BoundActions A) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<true>(nf, counts, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk);
+}
+
+// k_bound_reset: one CTA before run [f0, f1) of a bound call with actions, launched only for runs that hold a frame whose stream
+// has a frame in an earlier run. Every such frame whose action (the run's copy, act) is PWPP_FRAME_RESET restores its stream's
+// constructor state: the StreamState only, as pwpp_reset_stream (the history sizes live in it). The run's streams are
+// pairwise distinct, so no two threads write one state.
+constexpr int BR_THREADS = 128;
+
+__global__ void __launch_bounds__(BR_THREADS) k_bound_reset(int f0, int f1, const int* __restrict__ act, const int* __restrict__ dep,
+                                                            const int* __restrict__ b_stream, const StreamState* __restrict__ init,
+                                                            StreamState* __restrict__ states) {
+  for (int f = f0 + (int) threadIdx.x; f < f1; f += BR_THREADS)
+    if (dep[f] && act[f] == PWPP_FRAME_RESET) states[b_stream[f]] = init[b_stream[f]];
 }
 
 // grid.x of a launch over frames with these sizes and steps

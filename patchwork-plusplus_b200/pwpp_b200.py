@@ -75,6 +75,7 @@ def load_library():
     lib.pwpp_host_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_host_results.restype = i32
     lib.pwpp_bind_host_to_device.argtypes = [i32]; lib.pwpp_bind_host_to_device.restype = i32
     lib.pwpp_bind_call.argtypes = [vp, i32, vp, vp, vp, vp, vp]; lib.pwpp_bind_call.restype = i32
+    lib.pwpp_bind_call_actions.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]; lib.pwpp_bind_call_actions.restype = i32
     lib.pwpp_run_bound_call.argtypes = [vp, vp]; lib.pwpp_run_bound_call.restype = i32
     lib.pwpp_bound_call_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_bound_call_results.restype = i32
     lib.pwpp_unbind_call.argtypes = [vp]; lib.pwpp_unbind_call.restype = i32
@@ -92,6 +93,11 @@ def bind_host_to_device(device: int) -> int:
 
 class PwppError(RuntimeError):
     pass
+
+
+# per-frame actions of a bound call and the status values they leave (PWPP_FRAME_* / PWPP_ACTION_INVALID of include/pwpp.h)
+FRAME_RUN, FRAME_SKIP, FRAME_RESET = 0, 1, 2
+FRAME_SKIPPED, ACTION_INVALID = 2, 3
 
 
 # sensor_msgs/PointField datatype codes (PWPP_FIELD_* of include/pwpp.h) of the numpy scalar types
@@ -163,6 +169,7 @@ class Engine:
         self._streams = []   # stream of every frame of the last call
         self._rec_dtypes = []   # record dtype of every frame of the last records call (uint8 rows of point_step for (buffer, layout) frames)
         self._bound = None      # (frames, counts, streams, sum of max_n) of the bound call
+        self._bound_actions = None   # its actions tensor (bind_call(actions=...)), kept alive while bound
 
     def close(self):
         if getattr(self, "_h", None):
@@ -276,23 +283,33 @@ class Engine:
                            dtypes=dtypes)
 
     # ---- bound call: frame sizes read on the GPU, capturable into a CUDA graph ----
-    def bind_call(self, frames, max_n, layouts, counts, streams=None):
+    def bind_call(self, frames, max_n, layouts, counts, streams=None, actions=None):
         """Binds a call whose frame sizes live on the device (pwpp_bind_call). Frame f is up to max_n[f] records of layouts[f] at
         `frames[f]` (a device address or a CUDA tensor, any alignment), its size counts[f] of `counts`, an int64 CUDA tensor of
-        nframes entries read by the GPU at every run. `streams` as for estimate_host (None: frame f on stream f). The tensors are
-        kept alive while the call is bound; their contents may change between runs."""
+        nframes entries read by the GPU at every run. `streams` as for estimate_host (None: frame f on stream f). `actions`: an
+        optional int32 CUDA tensor of nframes per-frame actions read by the GPU at every run (pwpp_bind_call_actions):
+        FRAME_RUN, FRAME_SKIP (the frame is left out, its stream keeps its state) or FRAME_RESET (reset the stream, then run the
+        frame). The tensors are kept alive while the call is bound; their contents may change between runs."""
         import torch
         nf = len(frames)
         if not (isinstance(counts, torch.Tensor) and counts.is_cuda and counts.dtype == torch.int64 and counts.is_contiguous()
                 and counts.numel() == nf):
             raise PwppError(f"counts must be a contiguous int64 CUDA tensor of {nf} entries")
+        if actions is not None and not (isinstance(actions, torch.Tensor) and actions.is_cuda and actions.dtype == torch.int32
+                                        and actions.is_contiguous() and actions.numel() == nf):
+            raise PwppError(f"actions must be a contiguous int32 CUDA tensor of {nf} entries")
         ids = np.arange(nf, dtype=np.int32) if streams is None else self._stream_table(streams, nf)
         ptrs = [int(fr.data_ptr()) if isinstance(fr, torch.Tensor) else int(fr) for fr in frames]
         p = (C.c_void_p * max(nf, 1))(*ptrs)
         n = (C.c_int64 * max(nf, 1))(*[int(k) for k in max_n])
         lays = (PwppPointLayout * max(nf, 1))(*layouts)
-        _check(self.lib.pwpp_bind_call(self._h, nf, ids.ctypes.data, p, n, lays, C.c_void_p(counts.data_ptr())))
+        if actions is None:
+            _check(self.lib.pwpp_bind_call(self._h, nf, ids.ctypes.data, p, n, lays, C.c_void_p(counts.data_ptr())))
+        else:
+            _check(self.lib.pwpp_bind_call_actions(self._h, nf, ids.ctypes.data, p, n, lays, C.c_void_p(counts.data_ptr()),
+                                                   C.c_void_p(actions.data_ptr())))
         self._bound = (list(frames), counts, ids.tolist(), sum(int(k) for k in max_n))
+        self._bound_actions = actions
 
     def run_bound_call(self, stream: int = 0):
         """Enqueues the bound call on CUDA stream `stream` (0: the ctx's own stream; inside torch.cuda.graph pass
@@ -351,6 +368,7 @@ class Engine:
     def unbind_call(self):
         _check(self.lib.pwpp_unbind_call(self._h))
         self._bound = None
+        self._bound_actions = None
 
     def _use_bound(self):
         """The host getters now serve the bound call: its frame sizes are fetched from the device when first needed."""
