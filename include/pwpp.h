@@ -368,6 +368,54 @@ int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const voi
 #define PWPP_ACTION_INVALID 3   /* d_status[f]: the frame's action was not a PWPP_FRAME_* value; it was skipped */
 int pwpp_bind_call_actions(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
                            const pwpp_point_layout* layouts, const int64_t* d_counts, const int32_t* d_actions);
+
+/* Scan rings of a bound call: a driver, a packet decoder or a DMA engine writes scan t + 1 into the next slot of a ring while
+ * scan t is consumed. With rings the address of every frame is picked on the GPU at every run or replay, so the bound call
+ * segments each scan in the slot where it was written, with no copy into a fixed buffer.
+ *
+ * pwpp_scan_ring: slot s of a ring holds d_counts[s] records starting at base + s * slot_stride (device memory, any alignment).
+ *
+ * pwpp_bind_call_rings: pwpp_bind_call_actions with the frames in rings. Frame f reads ring rings[f] (descriptors are copied at
+ * bind time) and d_slots[f], a device int32 array of nframes slot numbers that the GPU reads at every run or replay, like the
+ * counts. d_actions as for pwpp_bind_call_actions (NULL: all RUN).
+ *   - Reading the slot. On every run or replay, frame f reads s = d_slots[f] once, in the run's first kernel, into a copy the ctx
+ *     owns (pwpp_bound_call_slots). It then reads rings[f].d_counts[s] and segments the records at base + s * slot_stride.
+ *     Everything else is as for pwpp_bind_call_actions: the count rule (a count outside [0, max_n[f]] gives
+ *     PWPP_COUNT_OUT_OF_RANGE and an empty frame), the actions, the record results, the freeze and pwpp_unbind_call.
+ *   - Precedence. A frame whose action skips it reads neither its slot nor a count (status PWPP_FRAME_SKIPPED or
+ *     PWPP_ACTION_INVALID, slot copy -1). Otherwise a slot outside [0, num_slots) gives PWPP_SLOT_OUT_OF_RANGE: the frame runs as
+ *     an empty frame and its stream advances as after an empty call, like an out-of-range count; a RESET still applies.
+ *     Otherwise the count rule applies.
+ *   - What is read. No byte outside [base, base + (num_slots - 1) * slot_stride + max_n[f] * point_step) is read, whatever
+ *     d_slots holds.
+ *   - Shared rings. Several frame entries may name the same ring, with identical descriptors: for example one sensor's backlog,
+ *     its stream bound twice, the second entry reading the next slot or skipped.
+ *   - The caller's obligation. Between a run's first kernel and the end of its last kernel (the record gather, when enabled), the
+ *     caller must not write a slot the run reads (its records or its count). Writing other slots, d_slots and other slots'
+ *     counts is allowed and does not affect the run.
+ *   - Bind-time checks, before anything is allocated, each message naming the frame (PWPP_ERR_INVALID_ARG): every check of
+ *     pwpp_bind_call with frames[f] = base and n = max_n; NULL rings, d_slots or d_counts; NULL base with max_n > 0;
+ *     num_slots < 1; slot_stride < max_n * point_step; a ring extent that overflows.
+ *   - pwpp_launch_count rises exactly as for the same call bound with pwpp_bind_call_actions: there is no extra launch.
+ *   - Identity. pwpp_bind_call_actions(frames, max_n, layouts, d_counts, d_actions) is this call with one-slot rings
+ *     {frames[f], max_n[f] * point_step, d_counts + f, 1} and d_slots all zero, bit for bit.
+ *   - Memory: 24 + 48 + 4 bytes per frame on the device, next to the bound call's other tables.
+ *
+ * pwpp_bound_call_slots: host-only. The ctx's copy of the slots the last run read, device int32[nframes] at a fixed address
+ * while the call stays bound: the slot each frame read (also an out-of-range one), -1 where the action skipped the frame; -1
+ * everywhere before the first run. PWPP_ERR_INVALID_ARG when no call is bound or it was bound without rings. */
+typedef struct pwpp_scan_ring {
+  const void* base;          /* device address of slot 0's first record (any alignment) */
+  int64_t slot_stride;       /* bytes from slot s to slot s + 1; >= max_n[f] * point_step of every frame bound to it */
+  const int64_t* d_counts;   /* device int64[num_slots]: the number of records in each slot, read by the GPU */
+  int32_t num_slots;         /* >= 1 */
+  int32_t _pad;
+} pwpp_scan_ring;
+#define PWPP_SLOT_OUT_OF_RANGE 4   /* d_status[f]: d_slots[f] < 0 or >= num_slots; the frame ran as an empty frame */
+int pwpp_bind_call_rings(pwpp_ctx* ctx, int nframes, const int32_t* streams, const pwpp_scan_ring* rings /* [nframes] */,
+                         const int64_t* max_n, const pwpp_point_layout* layouts, const int32_t* d_slots /* device [nframes] */,
+                         const int32_t* d_actions /* NULL: all RUN */);
+int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read);
 int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream);
 int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int64_t** d_offsets, const int32_t** d_num_ground,
                             const int32_t** d_status);

@@ -23,6 +23,7 @@
 using namespace pwpp;
 
 static_assert(sizeof(BinFit) == sizeof(pwpp_bin_result), "BinFit must mirror pwpp_bin_result");
+static_assert(sizeof(pwpp_scan_ring) == 32, "pwpp_scan_ring is a 32-byte record");
 
 namespace {
 
@@ -236,6 +237,7 @@ struct pwpp_ctx {
     std::vector<long long> rec_part_off;    // [F+1] byte offsets of every frame's region in each part buffer
     const int* d_actions = nullptr;         // the caller's device actions (pwpp_bind_call_actions), NULL: none
     std::vector<char> reset_run;            // [runs] the run holds a frame whose stream ran in an earlier run: k_bound_reset
+    const int* d_slots = nullptr;           // the caller's device slots (pwpp_bind_call_rings), NULL: no rings
   } bound;
   int scratch_slots = 0;                  // state / history slots after the streams' (pwpp_bind_call_actions), kept after unbind
   DevBuf<long long, false> d_bmax;        // [F] max_n
@@ -247,6 +249,9 @@ struct pwpp_ctx {
   DevBuf<int, false> d_rec_counts;        // [F][2]: ground, non-ground records of every frame of the last run
   DevBuf<int, false> d_bscratch, d_bdep;  // [F] with actions: scratch slot of every frame; its stream has a frame in an earlier run
   DevBuf<int, false> d_bact;              // [F] the run's copy of the actions
+  DevBuf<BoundRing, false> d_bring;       // [F] with rings: every frame's ring
+  DevBuf<int, false> d_bslot;             // [F] the run's copy of the slots
+  DevBuf<RecordFrame, false> d_brun;      // [F] the run's record table (d_brec with every frame's slot applied)
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
   struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
@@ -992,6 +997,7 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
   ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
   ctx->d_bscratch.release(); ctx->d_bdep.release(); ctx->d_bact.release();
+  ctx->d_bring.release(); ctx->d_bslot.release(); ctx->d_brun.release();
   if (ctx->ev_rec_off) cudaEventDestroy(ctx->ev_rec_off);
   ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
   ctx->h_out_idx.release(); ctx->h_counts.release();
@@ -1419,17 +1425,40 @@ int pwpp_bind_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const voi
   return pwpp_bind_call_actions(ctx, nframes, streams, frames, max_n, layouts, d_counts, nullptr);
 }
 
+// The checks of a ring-bound call beyond those of pwpp_bind_call (frames[f] = rings[f].base): the ring of every frame.
+static int check_rings(int nframes, const pwpp_scan_ring* rings, const int64_t* max_n, const pwpp_point_layout* layouts) {
+  for (int f = 0; f < nframes; ++f) {
+    const std::string fr = "frame " + std::to_string(f) + ": ";
+    const pwpp_scan_ring& R = rings[f];
+    const long long bytes = max_n[f] * layouts[f].point_step;   // (max_n < 2^31 and point_step <= PWPP_MAX_POINT_STEP: no overflow)
+    if (!R.d_counts) return fail(PWPP_ERR_INVALID_ARG, fr + "ring d_counts is NULL");
+    if (R.num_slots < 1) return fail(PWPP_ERR_INVALID_ARG, fr + "ring num_slots " + std::to_string(R.num_slots) + " < 1");
+    if (R.slot_stride < bytes)
+      return fail(PWPP_ERR_INVALID_ARG, fr + "ring slot_stride " + std::to_string(R.slot_stride) + " < max_n * point_step = " + std::to_string(bytes));
+    // the kernels form base + s * slot_stride in 64 bits: the extent and its end address must not overflow
+    const __int128 extent = (__int128) (R.num_slots - 1) * R.slot_stride + bytes;
+    if (extent > (__int128) INT64_MAX || (__int128) (uintptr_t) R.base + extent > (__int128) UINTPTR_MAX)
+      return fail(PWPP_ERR_INVALID_ARG, fr + "the ring's extent (num_slots - 1) * slot_stride + max_n * point_step overflows");
+  }
+  return PWPP_OK;
+}
+
+// The bind of pwpp_bind_call, pwpp_bind_call_actions and pwpp_bind_call_rings. rings is NULL for the first two; with rings,
+// frames[f] is rings[f].base and d_counts is unused.
 // With actions: frame f of run r gets scratch slot num_streams + (f - runs[r]) (distinct inside a run), and dep[f] says whether
 // its stream has a frame in an earlier run (then a RESET of f waits for that run: k_bound_reset before f's run).
-int pwpp_bind_call_actions(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
-                           const pwpp_point_layout* layouts, const int64_t* d_counts, const int32_t* d_actions) {
+static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
+                          const pwpp_point_layout* layouts, const int64_t* d_counts, const int32_t* d_actions, const pwpp_scan_ring* rings,
+                          const int32_t* d_slots) {
   int rc = check_records_call(ctx, nframes, streams, frames, max_n, layouts);
   if (rc) return rc;
   if (ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "a call is already bound (pwpp_unbind_call releases it)");
-  if (!d_counts) return fail(PWPP_ERR_INVALID_ARG, "d_counts is NULL");
+  if (!rings && !d_counts) return fail(PWPP_ERR_INVALID_ARG, "d_counts is NULL");
+  if (rings && (rc = check_rings(nframes, rings, max_n, layouts))) return rc;
   pwpp_ctx::Bound b;
   b.nf = nframes;
   b.d_counts = reinterpret_cast<const long long*>(d_counts);
+  b.d_slots = d_slots;
   b.cap_pt_off.assign(nframes + 1, 0);
   b.cap_chunk_off.assign(nframes + 1, 0);
   long long chunks = 0;
@@ -1515,10 +1544,36 @@ int pwpp_bind_call_actions(pwpp_ctx* ctx, int nframes, const int32_t* streams, c
   CU_TRY(cudaMemcpy(ctx->d_bpset.p, b.frame_set.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
   CU_TRY(cudaMemcpy(ctx->d_brec.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
   CU_TRY(cudaMemset(ctx->d_bstatus.p, 0, (size_t) nframes * sizeof(int)));
+  if (rings) {
+    std::vector<BoundRing> ring(nframes);
+    for (int f = 0; f < nframes; ++f)
+      ring[f] = BoundRing{reinterpret_cast<const long long*>(rings[f].d_counts), (long long) rings[f].slot_stride, (int) rings[f].num_slots, 0};
+    CU_TRY(ctx->d_bring.reserve(nframes));
+    CU_TRY(ctx->d_bslot.reserve(nframes));
+    CU_TRY(ctx->d_brun.reserve(nframes));
+    CU_TRY(cudaMemcpy(ctx->d_bring.p, ring.data(), (size_t) nframes * sizeof(BoundRing), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemcpy(ctx->d_brun.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemset(ctx->d_bslot.p, 0xff, (size_t) nframes * sizeof(int)));   // -1: no run yet
+  }
   CU_TRY(cudaDeviceSynchronize());
   b.on = true;
   ctx->bound = std::move(b);
   return PWPP_OK;
+}
+
+int pwpp_bind_call_actions(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
+                           const pwpp_point_layout* layouts, const int64_t* d_counts, const int32_t* d_actions) {
+  return bind_call_impl(ctx, nframes, streams, frames, max_n, layouts, d_counts, d_actions, nullptr, nullptr);
+}
+
+int pwpp_bind_call_rings(pwpp_ctx* ctx, int nframes, const int32_t* streams, const pwpp_scan_ring* rings, const int64_t* max_n,
+                         const pwpp_point_layout* layouts, const int32_t* d_slots, const int32_t* d_actions) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!rings) return fail(PWPP_ERR_INVALID_ARG, "rings is NULL");
+  if (!d_slots) return fail(PWPP_ERR_INVALID_ARG, "d_slots is NULL");
+  std::vector<const void*> frames(std::max(nframes, 1), nullptr);
+  for (int f = 0; f < nframes; ++f) frames[f] = rings[f].base;
+  return bind_call_impl(ctx, nframes, streams, frames.data(), max_n, layouts, nullptr, d_actions, rings, d_slots);
 }
 
 // One table launch, one unpack launch (capacities with points), then every run through launch_range_impl with grids sized for
@@ -1538,8 +1593,18 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   ctx->frame_set = b.frame_set;
   ctx->chunk_off = b.cap_chunk_off;
   ctx->pt_off = b.cap_pt_off;
-  if (b.d_actions) {
-    const BoundActions A{b.d_actions, ctx->d_bact.p, ctx->d_bscratch.p, ctx->d_bdep.p, ctx->d_states_init.p, ctx->d_states.p};
+  const BoundActions A{b.d_actions, ctx->d_bact.p, ctx->d_bscratch.p, ctx->d_bdep.p, ctx->d_states_init.p, ctx->d_states.p};
+  const RecordFrame* recs = ctx->d_brec.p;   // the record table the unpack and the gather read
+  if (b.d_slots) {
+    const BoundRings G{b.d_slots, ctx->d_bslot.p, ctx->d_bring.p, ctx->d_brec.p, ctx->d_brun.p};
+    if (b.d_actions)
+      k_bound_table_rings_actions<<<1, BT_THREADS, 0, s>>>(nf, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                                           ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p, A, G);
+    else
+      k_bound_table_rings<<<1, BT_THREADS, 0, s>>>(nf, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                                   ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p, G);
+    recs = ctx->d_brun.p;
+  } else if (b.d_actions) {
     k_bound_table_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
                                                    ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p, A);
   } else {
@@ -1548,7 +1613,7 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   }
   ++ctx->launches;
   if (b.unpack_gx > 0) {
-    k_unpack_records<<<dim3((unsigned) b.unpack_gx, (unsigned) nf), REC_THREADS, 0, s>>>(ctx->d_brec.p, ctx->d_pt_off.p, ctx->d_in.p);
+    k_unpack_records<<<dim3((unsigned) b.unpack_gx, (unsigned) nf), REC_THREADS, 0, s>>>(recs, ctx->d_pt_off.p, ctx->d_in.p);
     ++ctx->launches;
   }
   CU_TRY(cudaGetLastError());
@@ -1564,7 +1629,7 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   if (b.rec_parts) {   // the record results: both parts' lists are where the runs' k_emit left them
     const int first = b.rec_parts == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.rec_parts == 3 ? 2 : 1;
     k_gather_record_parts<<<dim3((unsigned) b.rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
-        ctx->d_brec.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, ctx->d_bpart_off.p, first, ctx->d_bground.p, ctx->d_bnonground.p,
+        recs, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, ctx->d_bpart_off.p, first, ctx->d_bground.p, ctx->d_bnonground.p,
         ctx->d_rec_counts.p);
     ++ctx->launches;
     CU_TRY(cudaGetLastError());
@@ -1586,6 +1651,14 @@ int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int6
   return PWPP_OK;
 }
 
+int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call_rings)");
+  if (!ctx->bound.d_slots) return fail(PWPP_ERR_INVALID_ARG, "the bound call has no rings (pwpp_bind_call_rings)");
+  if (d_slots_read) *d_slots_read = ctx->d_bslot.p;
+  return PWPP_OK;
+}
+
 int pwpp_unbind_call(pwpp_ctx* ctx) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound");
@@ -1594,6 +1667,7 @@ int pwpp_unbind_call(pwpp_ctx* ctx) {
   ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
   ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
   ctx->d_bscratch.release(); ctx->d_bdep.release(); ctx->d_bact.release();
+  ctx->d_bring.release(); ctx->d_bslot.release(); ctx->d_brun.release();
   ctx->bound = pwpp_ctx::Bound();
   return PWPP_OK;
 }

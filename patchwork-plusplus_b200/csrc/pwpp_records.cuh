@@ -149,6 +149,12 @@ inline RecordFrame record_frame(const pwpp_point_layout& L, const void* src) {
 // the empty frame's update there and the real stream is never touched. A RESET frame whose stream has no frame in an earlier
 // run (dep[f] == 0) gets its stream's constructor state here, before any run; the others are reset by k_bound_reset right
 // before their run.
+//
+// With scan rings (pwpp_bind_call_rings), k_bound_table_rings / k_bound_table_rings_actions also pick every frame's address:
+// a frame that runs reads its slot s = slots[f] once into the ctx's copy slot[f] (-1 for a skipped frame), takes its count
+// from its ring's counts[s] and writes the run's record table entry brun[f] = the bound entry brec[f] with src = base +
+// s * stride. A slot outside [0, num_slots) makes an empty frame with status PWPP_SLOT_OUT_OF_RANGE; skipped frames and those
+// keep src = base with n = 0, so nothing is read. The unpack and the record gather of the run read brun.
 constexpr int BT_THREADS = 1024;
 
 struct BoundActions {
@@ -170,11 +176,42 @@ __device__ __forceinline__ int bt_action(const BoundActions& A, int f) {
 }
 __device__ __forceinline__ bool bt_runs(int a) { return a == PWPP_FRAME_RUN || a == PWPP_FRAME_RESET; }
 
-template <bool Actions>
+// one frame's ring (uploaded at bind time, next to max_n and the stream table)
+struct BoundRing {
+  const long long* counts;       // the caller's device counts [num_slots]
+  long long stride;              // bytes from slot s to slot s + 1
+  int num_slots;
+  int pad;
+};
+static_assert(sizeof(BoundRing) == 24, "BoundRing is uploaded as a 24-byte record");
+
+struct BoundRings {
+  const int* slots;              // the caller's device slots [nf]
+  int* slot;                     // the ctx's copy [nf]: the slot each frame read, -1 for a skipped frame
+  const BoundRing* ring;         // [nf]
+  const RecordFrame* brec;       // the bound record table (src: slot 0)
+  RecordFrame* brun;             // the run's record table
+};
+
+__device__ __forceinline__ bool bt_slot_ok(int s, const BoundRing& R) { return s >= 0 && s < R.num_slots; }
+
+// frame f's count for the first pass: counts[f], or with rings its slot's count (the slot read once and copied; -1, an empty
+// frame, for a slot out of range)
+template <bool Rings>
+__device__ __forceinline__ long long bt_count(const long long* __restrict__ counts, const BoundRings& G, int f) {
+  if (!Rings) return counts[f];
+  const int s = G.slots[f];
+  G.slot[f] = s;
+  const BoundRing R = G.ring[f];
+  return bt_slot_ok(s, R) ? R.counts[s] : -1;
+}
+
+template <bool Actions, bool Rings = false>
 __device__ __forceinline__ void bound_table_body(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
                                                  const int* __restrict__ b_stream, const int* __restrict__ b_pset, long long* __restrict__ pt_off,
                                                  int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
-                                                 int* __restrict__ status, const BoundActions& A, long long* s_pts, int* s_chk) {
+                                                 int* __restrict__ status, const BoundActions& A, long long* s_pts, int* s_chk,
+                                                 const BoundRings& G = BoundRings{}) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int per = (nf + BT_THREADS - 1) / BT_THREADS;
   const int f0 = tid * per < nf ? tid * per : nf;
@@ -184,8 +221,10 @@ __device__ __forceinline__ void bound_table_body(int nf, const long long* __rest
   for (int f = f0; f < f1; ++f) {
     long long n = 0;
     if (bt_runs(bt_action<Actions>(A, f))) {
-      const long long c = counts[f];
+      const long long c = bt_count<Rings>(counts, G, f);
       n = (c >= 0 && c <= max_n[f]) ? c : 0;
+    } else if (Rings) {
+      G.slot[f] = -1;
     }
     own_pts += n;
     own_chk += (int) ((n + CHUNK_PTS - 1) / CHUNK_PTS);
@@ -222,16 +261,33 @@ __device__ __forceinline__ void bound_table_body(int nf, const long long* __rest
         status[f] = a == PWPP_FRAME_SKIP ? PWPP_FRAME_SKIPPED : PWPP_ACTION_INVALID;
         stream[f] = A.scratch[f];
         pset[f] = b_pset[f];
+        if (Rings) G.brun[f] = G.brec[f];
         continue;
       }
       if (a == PWPP_FRAME_RESET && !A.dep[f]) A.states[b_stream[f]] = A.init[b_stream[f]];
     }
-    const long long c = counts[f];
+    long long c;
+    int bad = PWPP_COUNT_OUT_OF_RANGE;
+    if (Rings) {
+      const int s = G.slot[f];   // this thread's own copy from the first pass
+      const BoundRing R = G.ring[f];
+      RecordFrame r = G.brec[f];
+      if (bt_slot_ok(s, R)) {
+        c = R.counts[s];
+        r.src += (long long) s * R.stride;
+      } else {
+        c = -1;
+        bad = PWPP_SLOT_OUT_OF_RANGE;
+      }
+      G.brun[f] = r;
+    } else {
+      c = counts[f];
+    }
     const bool ok = c >= 0 && c <= max_n[f];
     const long long n = ok ? c : 0;
     pt_off[f] = p;
     chunk_off[f] = q;
-    status[f] = ok ? 0 : PWPP_COUNT_OUT_OF_RANGE;
+    status[f] = ok ? 0 : bad;
     stream[f] = b_stream[f];
     pset[f] = b_pset[f];
     p += n;
@@ -256,6 +312,24 @@ __global__ void __launch_bounds__(BT_THREADS) k_bound_table_actions(int nf, cons
   __shared__ long long s_pts[BT_THREADS / 32];
   __shared__ int s_chk[BT_THREADS / 32];
   bound_table_body<true>(nf, counts, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk);
+}
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table_rings(int nf, const long long* __restrict__ max_n, const int* __restrict__ b_stream,
+                                                                  const int* __restrict__ b_pset, long long* __restrict__ pt_off,
+                                                                  int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
+                                                                  int* __restrict__ status, const BoundRings G) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<false, true>(nf, nullptr, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, BoundActions{}, s_pts, s_chk, G);
+}
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table_rings_actions(int nf, const long long* __restrict__ max_n, const int* __restrict__ b_stream,
+                                                                          const int* __restrict__ b_pset, long long* __restrict__ pt_off,
+                                                                          int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
+                                                                          int* __restrict__ status, const BoundActions A, const BoundRings G) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<true, true>(nf, nullptr, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk, G);
 }
 
 // k_bound_reset: one CTA before run [f0, f1) of a bound call with actions, launched only for runs that hold a frame whose stream

@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from pwpp_ctypes import PwppBinResult, PwppParams, PwppPointLayout, PwppState, default_params  # noqa: F401
+from pwpp_ctypes import PwppBinResult, PwppParams, PwppPointLayout, PwppScanRing, PwppState, default_params  # noqa: F401
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PWPP_LIB") or os.path.join(_HERE, "lib", "libpwpp_b200.so")   # PWPP_LIB: a diagnostic build of the same library
@@ -76,6 +76,8 @@ def load_library():
     lib.pwpp_bind_host_to_device.argtypes = [i32]; lib.pwpp_bind_host_to_device.restype = i32
     lib.pwpp_bind_call.argtypes = [vp, i32, vp, vp, vp, vp, vp]; lib.pwpp_bind_call.restype = i32
     lib.pwpp_bind_call_actions.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]; lib.pwpp_bind_call_actions.restype = i32
+    lib.pwpp_bind_call_rings.argtypes = [vp, i32, vp, C.POINTER(PwppScanRing), vp, vp, vp, vp]; lib.pwpp_bind_call_rings.restype = i32
+    lib.pwpp_bound_call_slots.argtypes = [vp, C.POINTER(vp)]; lib.pwpp_bound_call_slots.restype = i32
     lib.pwpp_run_bound_call.argtypes = [vp, vp]; lib.pwpp_run_bound_call.restype = i32
     lib.pwpp_bound_call_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_bound_call_results.restype = i32
     lib.pwpp_unbind_call.argtypes = [vp]; lib.pwpp_unbind_call.restype = i32
@@ -98,6 +100,7 @@ class PwppError(RuntimeError):
 # per-frame actions of a bound call and the status values they leave (PWPP_FRAME_* / PWPP_ACTION_INVALID of include/pwpp.h)
 FRAME_RUN, FRAME_SKIP, FRAME_RESET = 0, 1, 2
 FRAME_SKIPPED, ACTION_INVALID = 2, 3
+SLOT_OUT_OF_RANGE = 4   # status of a ring-bound frame whose slot is outside its ring (PWPP_SLOT_OUT_OF_RANGE)
 
 
 # sensor_msgs/PointField datatype codes (PWPP_FIELD_* of include/pwpp.h) of the numpy scalar types
@@ -170,6 +173,7 @@ class Engine:
         self._rec_dtypes = []   # record dtype of every frame of the last records call (uint8 rows of point_step for (buffer, layout) frames)
         self._bound = None      # (frames, counts, streams, sum of max_n) of the bound call
         self._bound_actions = None   # its actions tensor (bind_call(actions=...)), kept alive while bound
+        self._bound_rings = None     # its ring tensors and slots (bind_call_rings), kept alive while bound
 
     def close(self):
         if getattr(self, "_h", None):
@@ -311,6 +315,69 @@ class Engine:
         self._bound = (list(frames), counts, ids.tolist(), sum(int(k) for k in max_n))
         self._bound_actions = actions
 
+    def bind_call_rings(self, rings, max_n, layouts, slots, streams=None, actions=None):
+        """Binds a call whose frames live in scan rings (pwpp_bind_call_rings): at every run or replay frame f reads slot
+        slots[f] of rings[f] and segments the records written there. A ring is (buffer, counts) or (buffer, counts, slot_stride):
+        buffer a contiguous CUDA tensor holding the slots (without slot_stride: its first dimension is the slot, e.g. uint8
+        (num_slots, slot_stride)), counts a contiguous int64 CUDA tensor of num_slots record counts read by the GPU, slot_stride
+        the bytes from one slot to the next. Frame f holds up to max_n[f] records of layouts[f]. `slots`: a contiguous int32 CUDA
+        tensor of nframes slot numbers read by the GPU at every run. `streams` and `actions` as for bind_call. The tensors are
+        kept alive while the call is bound; the slots, the counts and the slots' contents may change between runs."""
+        import torch
+        nf = len(rings)
+
+        def cuda_vec(t, dtype, n, what):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dtype and t.is_contiguous() and (n is None or t.numel() == n)):
+                raise PwppError(f"{what} must be a contiguous {str(dtype).replace('torch.', '')} CUDA tensor" + (f" of {n} entries" if n else ""))
+        cuda_vec(slots, torch.int32, nf, "slots")
+        if actions is not None:
+            cuda_vec(actions, torch.int32, nf, "actions")
+        if len(max_n) != nf or len(layouts) != nf:
+            raise PwppError(f"max_n and layouts must name one entry per ring ({nf})")
+        descs = (PwppScanRing * max(nf, 1))()
+        for f, ring in enumerate(rings):
+            if not isinstance(ring, tuple) or len(ring) not in (2, 3):
+                raise PwppError(f"ring {f}: a ring is (buffer, counts) or (buffer, counts, slot_stride)")
+            buf, counts = ring[:2]
+            if not (isinstance(buf, torch.Tensor) and buf.is_cuda and buf.is_contiguous()):
+                raise PwppError(f"ring {f}: buffer must be a contiguous CUDA tensor")
+            cuda_vec(counts, torch.int64, None, f"ring {f}: counts")
+            num_slots = counts.numel()
+            nbytes = buf.numel() * buf.element_size()
+            if len(ring) == 3:
+                stride = int(ring[2])
+            else:
+                if buf.dim() < 1 or buf.shape[0] != num_slots:
+                    raise PwppError(f"ring {f}: buffer's first dimension must be the {num_slots} slots of counts")
+                stride = nbytes // num_slots if num_slots else 0
+            need = (num_slots - 1) * stride + int(max_n[f]) * layouts[f].point_step
+            if num_slots >= 1 and int(max_n[f]) > 0 and need > nbytes:
+                raise PwppError(f"ring {f}: {num_slots} slots of stride {stride} with max_n {int(max_n[f])} reach {need} bytes, "
+                                f"past the buffer's {nbytes}")
+            descs[f].base, descs[f].slot_stride = buf.data_ptr(), stride
+            descs[f].d_counts, descs[f].num_slots = counts.data_ptr(), num_slots
+        ids = np.arange(nf, dtype=np.int32) if streams is None else self._stream_table(streams, nf)
+        n = (C.c_int64 * max(nf, 1))(*[int(k) for k in max_n])
+        lays = (PwppPointLayout * max(nf, 1))(*layouts)
+        _check(self.lib.pwpp_bind_call_rings(self._h, nf, ids.ctypes.data, descs, n, lays, C.c_void_p(slots.data_ptr()),
+                                             C.c_void_p(actions.data_ptr() if actions is not None else None)))
+        self._bound = ([r[0] for r in rings], None, ids.tolist(), sum(int(k) for k in max_n))
+        self._bound_actions = actions
+        self._bound_rings = (list(rings), slots)
+
+    def bound_call_slots(self):
+        """Torch view (int32 [nframes]) of the slots the last run read (pwpp_bound_call_slots): the run's own copy, -1 where the
+        action skipped the frame. Fixed address while the call is bound."""
+        import torch
+        a = C.c_void_p()
+        _check(self.lib.pwpp_bound_call_slots(self._h, C.byref(a)))
+        nf = len(self._bound[0])
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr, n):
+                self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<i4", "data": (ptr, False), "version": 3, "strides": None}
+        return torch.as_tensor(_View(a.value, nf), device="cuda")
+
     def run_bound_call(self, stream: int = 0):
         """Enqueues the bound call on CUDA stream `stream` (0: the ctx's own stream; inside torch.cuda.graph pass
         torch.cuda.current_stream().cuda_stream). No host synchronisation: it may be captured and replayed."""
@@ -369,6 +436,7 @@ class Engine:
         _check(self.lib.pwpp_unbind_call(self._h))
         self._bound = None
         self._bound_actions = None
+        self._bound_rings = None
 
     def _use_bound(self):
         """The host getters now serve the bound call: its frame sizes are fetched from the device when first needed."""

@@ -51,3 +51,8 @@ class PwppBinResult(C.Structure):
 class PwppPointLayout(C.Structure):
     """Mirror of `pwpp_point_layout` (include/pwpp.h): the record layout of a frame for pwpp_estimate_*_records."""
     _fields_ = [("point_step", C.c_int32), ("offset", C.c_int32 * 4), ("datatype", C.c_int32 * 4)]
+
+
+class PwppScanRing(C.Structure):
+    """Mirror of `pwpp_scan_ring` (include/pwpp.h): a ring of scan slots in device memory for pwpp_bind_call_rings."""
+    _fields_ = [("base", C.c_void_p), ("slot_stride", C.c_int64), ("d_counts", C.c_void_p), ("num_slots", C.c_int32), ("_pad", C.c_int32)]
