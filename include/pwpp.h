@@ -424,7 +424,57 @@ int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int6
 int pwpp_bind_record_results(pwpp_ctx* ctx, int parts /* PWPP_PART_* bits: 1, 2 or 3 */);
 int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void** d_nonground, const int64_t** h_offsets,
                               const int32_t** d_counts);
-/* Releases the bound call and its record results (PWPP_ERR_INVALID_ARG when none is bound). Its index results stay readable
+
+/* Getter results of the bound call: what the reference's other getters return (getGround / getNonground, getCenters /
+ * getNormals, getHeight and the adaptive thresholds, H:154-163), at fixed device addresses, for a graph whose next stage takes
+ * float32 xyz, the patch planes or the sensor height without a host round trip. Every value is one a host getter returns.
+ *
+ * pwpp_bind_getter_results: enables them for the bound call. what is a bit set of PWPP_GETTER_GROUND_XYZ,
+ * PWPP_GETTER_NONGROUND_XYZ and PWPP_GETTER_STATE, in [1, 7]. Host work like pwpp_bind_record_results (it reserves the buffers,
+ * then synchronizes), so it is not capturable; graphs captured before it do not write these results. PWPP_ERR_INVALID_ARG when
+ * no call is bound, for what outside [1, 7], and when they are already enabled (one setting per bind: pwpp_unbind_call releases
+ * the buffers, and a later bind starts with them off).
+ *
+ * pwpp_bound_getter_results: host-only; fills *out with fixed device pointers (PWPP_ERR_INVALID_ARG when no call is bound).
+ *   - xyz: ground_xyz and nonground_xyz are float32 rows of 3 (NULL for a part that is not enabled), sum(max_n) rows each.
+ *     Frame f's rows start at row h_row_off[f] of both (host int64[nframes + 1], the prefix sum of max_n). xyz_counts is
+ *     device int32[2 nframes]: ground count, then non-ground count of every frame (NULL when no xyz part is enabled). Row k of a
+ *     part is row k of pwpp_copy_ground_xyz / pwpp_copy_nonground_xyz of that frame after the same run, bit for bit, in the list
+ *     order the call was bound with (for an RNR-rejected point, its original z). Rows past a count are never written; a
+ *     skipped frame or one whose count or slot was out of range has counts 0.
+ *   - Patches: centers and normals (float32 rows of 3), num_patches (device int32[nframes]) and patch_row_stride. Frame f's
+ *     num_patches[f] rows start at row f * patch_row_stride, bit for bit what pwpp_copy_centers / pwpp_copy_normals return.
+ *     They are k_gle's own output: always available while a call is bound, with no enable bit and no launch.
+ *   - State: states is device pwpp_state[nframes] (NULL when not enabled). Row f is the state of frame f's stream immediately
+ *     after frame f: what pwpp_get_state on that stream would return had the call stopped there. A skipped frame (SKIP or an
+ *     invalid action) gets its stream's state as its earlier frames of the call left it (the real stream, never a scratch
+ *     slot); an out-of-range count or slot, the state after the empty frame; a RESET frame, the state after the reset and then
+ *     the frame. A stream bound twice (a backlog) has two rows that differ as after two direct calls.
+ * Rules:
+ *   - Valid until the next call or replay. Direct calls between runs never write the xyz or state buffers; they do overwrite
+ *     the patch rows and counts, like the index lists.
+ *   - pwpp_launch_count rises, per pwpp_run_bound_call, by one xyz gather launch when either xyz part is enabled (after the
+ *     last run's output kernel, also when every max_n is 0), and by one state launch after each run of the call (a run: a
+ *     maximal group of consecutive frames with pairwise distinct streams) when the state is enabled. Nothing for the patches.
+ *   - Memory: 12 sum(max_n) bytes per enabled xyz part plus 8 nframes bytes of counts and 8 (nframes + 1) bytes of row
+ *     offsets when either is enabled, and sizeof(pwpp_state) nframes bytes for the state. */
+#define PWPP_GETTER_GROUND_XYZ 1
+#define PWPP_GETTER_NONGROUND_XYZ 2
+#define PWPP_GETTER_STATE 4
+typedef struct pwpp_bound_getters {
+  const float* ground_xyz;        /* device float32 [sum(max_n)][3], or NULL */
+  const float* nonground_xyz;     /* device float32 [sum(max_n)][3], or NULL */
+  const int64_t* h_row_off;       /* host int64 [nframes + 1]: frame f's rows start at row h_row_off[f] */
+  const int32_t* xyz_counts;      /* device int32 [nframes][2]: ground, non-ground; NULL without an xyz part */
+  const float* centers;           /* device float32 rows of 3: frame f's patches start at row f * patch_row_stride */
+  const float* normals;
+  const int32_t* num_patches;     /* device int32 [nframes] */
+  int64_t patch_row_stride;
+  const pwpp_state* states;       /* device [nframes], or NULL */
+} pwpp_bound_getters;
+int pwpp_bind_getter_results(pwpp_ctx* ctx, int what /* PWPP_GETTER_* bits, 1..7 */);
+int pwpp_bound_getter_results(pwpp_ctx* ctx, pwpp_bound_getters* out);
+/* Releases the bound call, its record results and its getter results (PWPP_ERR_INVALID_ARG when none is bound). Its index results stay readable
  * until the next call. */
 int pwpp_unbind_call(pwpp_ctx* ctx);
 

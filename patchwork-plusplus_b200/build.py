@@ -104,6 +104,12 @@ def build_examples(force=False):
     if force or _newer(out8, [src8] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out8, src8])
+    # the kernels of a bound call's getter results, the same way (GPU cases of tests/test_bound_getters_backends.py)
+    src9 = os.path.join(REPO, "tests", "gpu_bound_getters_probe.cu")
+    out9 = os.path.join(LIB, "libpwpp_bound_getters_probe.so")
+    if force or _newer(out9, [src9] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out9, src9])
     return out
 
 

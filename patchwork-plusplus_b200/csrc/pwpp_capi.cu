@@ -17,6 +17,7 @@
 #include "pwpp.h"
 #include "pwpp_kernels.cuh"
 #include "pwpp_records.cuh"
+#include "pwpp_getters.cuh"
 #include "pwpp_tuning.h"
 #include "pwpp_host.hpp"
 
@@ -24,6 +25,7 @@ using namespace pwpp;
 
 static_assert(sizeof(BinFit) == sizeof(pwpp_bin_result), "BinFit must mirror pwpp_bin_result");
 static_assert(sizeof(pwpp_scan_ring) == 32, "pwpp_scan_ring is a 32-byte record");
+static_assert(sizeof(pwpp_state) == 104, "pwpp_state is a 104-byte record");
 
 namespace {
 
@@ -238,6 +240,8 @@ struct pwpp_ctx {
     const int* d_actions = nullptr;         // the caller's device actions (pwpp_bind_call_actions), NULL: none
     std::vector<char> reset_run;            // [runs] the run holds a frame whose stream ran in an earlier run: k_bound_reset
     const int* d_slots = nullptr;           // the caller's device slots (pwpp_bind_call_rings), NULL: no rings
+    int getters = 0;                        // getter results (pwpp_bind_getter_results): PWPP_GETTER_* bits, 0 = off
+    long long xyz_gx = 0;                   // grid.x of k_gather_xyz_parts, from the capacities
   } bound;
   int scratch_slots = 0;                  // state / history slots after the streams' (pwpp_bind_call_actions), kept after unbind
   DevBuf<long long, false> d_bmax;        // [F] max_n
@@ -252,6 +256,10 @@ struct pwpp_ctx {
   DevBuf<BoundRing, false> d_bring;       // [F] with rings: every frame's ring
   DevBuf<int, false> d_bslot;             // [F] the run's copy of the slots
   DevBuf<RecordFrame, false> d_brun;      // [F] the run's record table (d_brec with every frame's slot applied)
+  DevBuf<float, false> d_bgxyz, d_bngxyz;  // getter results: [sum(max_n)][3] ground / non-ground xyz, frame f from row cap_pt_off[f]
+  DevBuf<long long, false> d_bxyz_off;    // [F+1] cap_pt_off
+  DevBuf<int, false> d_xyz_counts;        // [F][2]: ground, non-ground xyz rows of every frame of the last run
+  DevBuf<pwpp_state, false> d_bstates;    // [F] the state of every frame's stream right after the frame
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
   struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
@@ -998,6 +1006,7 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
   ctx->d_bscratch.release(); ctx->d_bdep.release(); ctx->d_bact.release();
   ctx->d_bring.release(); ctx->d_bslot.release(); ctx->d_brun.release();
+  ctx->d_bgxyz.release(); ctx->d_bngxyz.release(); ctx->d_bxyz_off.release(); ctx->d_xyz_counts.release(); ctx->d_bstates.release();
   if (ctx->ev_rec_off) cudaEventDestroy(ctx->ev_rec_off);
   ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
   ctx->h_out_idx.release(); ctx->h_counts.release();
@@ -1625,12 +1634,26 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     }
     rc = launch_range_impl(ctx, b.runs[r], b.runs[r + 1] - b.runs[r], ctx->d_in.p, b.has_intensity, s, false, b.run_chunks[r]);
     if (rc) return rc;
+    if (b.getters & PWPP_GETTER_STATE) {   // before a later run moves the run's streams
+      const int len = b.runs[r + 1] - b.runs[r];
+      k_bound_states<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], ctx->d_bstream.p, ctx->d_states.p, ctx->d_bstates.p);
+      ++ctx->launches;
+      CU_TRY(cudaGetLastError());
+    }
   }
   if (b.rec_parts) {   // the record results: both parts' lists are where the runs' k_emit left them
     const int first = b.rec_parts == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.rec_parts == 3 ? 2 : 1;
     k_gather_record_parts<<<dim3((unsigned) b.rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
         recs, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, ctx->d_bpart_off.p, first, ctx->d_bground.p, ctx->d_bnonground.p,
         ctx->d_rec_counts.p);
+    ++ctx->launches;
+    CU_TRY(cudaGetLastError());
+  }
+  if (b.getters & (PWPP_GETTER_GROUND_XYZ | PWPP_GETTER_NONGROUND_XYZ)) {   // the xyz of both lists, from the unpacked points
+    const int parts = b.getters & 3, first = parts == PWPP_GETTER_NONGROUND_XYZ ? 1 : 0, nparts = parts == 3 ? 2 : 1;
+    k_gather_xyz_parts<<<dim3((unsigned) b.xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
+        ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, ctx->d_bxyz_off.p, first, ctx->d_bgxyz.p, ctx->d_bngxyz.p,
+        ctx->d_xyz_counts.p);
     ++ctx->launches;
     CU_TRY(cudaGetLastError());
   }
@@ -1668,6 +1691,7 @@ int pwpp_unbind_call(pwpp_ctx* ctx) {
   ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
   ctx->d_bscratch.release(); ctx->d_bdep.release(); ctx->d_bact.release();
   ctx->d_bring.release(); ctx->d_bslot.release(); ctx->d_brun.release();
+  ctx->d_bgxyz.release(); ctx->d_bngxyz.release(); ctx->d_bxyz_off.release(); ctx->d_xyz_counts.release(); ctx->d_bstates.release();
   ctx->bound = pwpp_ctx::Bound();
   return PWPP_OK;
 }
@@ -1707,6 +1731,52 @@ int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void**
   if (d_nonground) *d_nonground = (b.rec_parts & PWPP_PART_NONGROUND) ? ctx->d_bnonground.p : nullptr;
   if (h_offsets) *h_offsets = reinterpret_cast<const int64_t*>(b.rec_part_off.data());
   if (d_counts) *d_counts = ctx->d_rec_counts.p;
+  return PWPP_OK;
+}
+
+int pwpp_bind_getter_results(pwpp_ctx* ctx, int what) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (what < 1 || what > 7) return fail(PWPP_ERR_INVALID_ARG, "what must be a non-empty set of PWPP_GETTER_GROUND_XYZ, PWPP_GETTER_NONGROUND_XYZ and PWPP_GETTER_STATE");
+  if (b.getters) return fail(PWPP_ERR_INVALID_ARG, "getter results are already enabled for the bound call");
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const int nf = b.nf;
+  const size_t rows = (size_t) std::max<long long>(b.cap_pt_off[nf], 1);
+  if (what & PWPP_GETTER_GROUND_XYZ) CU_TRY(ctx->d_bgxyz.reserve(3 * rows));
+  if (what & PWPP_GETTER_NONGROUND_XYZ) CU_TRY(ctx->d_bngxyz.reserve(3 * rows));
+  if (what & (PWPP_GETTER_GROUND_XYZ | PWPP_GETTER_NONGROUND_XYZ)) {
+    CU_TRY(ctx->d_bxyz_off.reserve(nf + 1));
+    CU_TRY(ctx->d_xyz_counts.reserve(2 * (size_t) nf));
+    CU_TRY(cudaMemcpy(ctx->d_bxyz_off.p, b.cap_pt_off.data(), (size_t) (nf + 1) * sizeof(long long), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemset(ctx->d_xyz_counts.p, 0, 2 * (size_t) nf * sizeof(int)));
+  }
+  if (what & PWPP_GETTER_STATE) {
+    CU_TRY(ctx->d_bstates.reserve(nf));
+    CU_TRY(cudaMemset(ctx->d_bstates.p, 0, (size_t) nf * sizeof(pwpp_state)));
+  }
+  CU_TRY(cudaDeviceSynchronize());
+  b.xyz_gx = xyz_parts_grid_x(b.cap_pt_off.data(), nf);
+  b.getters = what;
+  return PWPP_OK;
+}
+
+int pwpp_bound_getter_results(pwpp_ctx* ctx, pwpp_bound_getters* out) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!out) return fail(PWPP_ERR_INVALID_ARG, "out is NULL");
+  const pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  *out = pwpp_bound_getters{};
+  out->ground_xyz = (b.getters & PWPP_GETTER_GROUND_XYZ) ? ctx->d_bgxyz.p : nullptr;
+  out->nonground_xyz = (b.getters & PWPP_GETTER_NONGROUND_XYZ) ? ctx->d_bngxyz.p : nullptr;
+  out->h_row_off = reinterpret_cast<const int64_t*>(b.cap_pt_off.data());
+  out->xyz_counts = (b.getters & 3) ? ctx->d_xyz_counts.p : nullptr;
+  out->centers = ctx->d_centers.p;
+  out->normals = ctx->d_normals.p;
+  out->num_patches = ctx->d_counts.p + b.nf;   // row 1 of the count rows of the bound call
+  out->patch_row_stride = ctx->gs.nbs;
+  out->states = (b.getters & PWPP_GETTER_STATE) ? ctx->d_bstates.p : nullptr;
   return PWPP_OK;
 }
 

@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from pwpp_ctypes import PwppBinResult, PwppParams, PwppPointLayout, PwppScanRing, PwppState, default_params  # noqa: F401
+from pwpp_ctypes import PwppBinResult, PwppBoundGetters, PwppParams, PwppPointLayout, PwppScanRing, PwppState, default_params  # noqa: F401
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PWPP_LIB") or os.path.join(_HERE, "lib", "libpwpp_b200.so")   # PWPP_LIB: a diagnostic build of the same library
@@ -84,6 +84,8 @@ def load_library():
     lib.pwpp_bind_record_results.argtypes = [vp, i32]; lib.pwpp_bind_record_results.restype = i32
     lib.pwpp_bound_record_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     lib.pwpp_bound_record_results.restype = i32
+    lib.pwpp_bind_getter_results.argtypes = [vp, i32]; lib.pwpp_bind_getter_results.restype = i32
+    lib.pwpp_bound_getter_results.argtypes = [vp, C.POINTER(PwppBoundGetters)]; lib.pwpp_bound_getter_results.restype = i32
     _lib = lib
     return lib
 
@@ -431,6 +433,54 @@ class Engine:
                 return None
             return torch.as_tensor(_View(ptr, (total,), "|u1"), device="cuda") if total > 0 else torch.empty(0, dtype=torch.uint8, device="cuda")
         return part(a.value), part(b.value), off, torch.as_tensor(_View(d.value, (nf, 2), "<i4"), device="cuda")
+
+    def bind_getter_results(self, ground_xyz: bool = True, nonground_xyz: bool = True, state: bool = True):
+        """Enables the bound call's getter results (pwpp_bind_getter_results): every later run_bound_call, and every graph
+        captured after this, also writes the ground and / or non-ground xyz of every frame and / or the state of every frame's
+        stream right after the frame into fixed device buffers. Host work that synchronizes: call it before a capture."""
+        what = (1 if ground_xyz else 0) | (2 if nonground_xyz else 0) | (4 if state else 0)
+        _check(self.lib.pwpp_bind_getter_results(self._h, what))
+
+    def bound_getter_results(self):
+        """Zero-copy views of the bound call's getter results (pwpp_bound_getter_results), as a dict. Fixed addresses while the
+        call is bound; valid after a run or replay until the next one.
+          ground_xyz, nonground_xyz: float32 CUDA tensors (sum(max_n), 3), None for a part that is not enabled;
+          row_off: int64 numpy [nframes + 1], frame f's rows start at row_off[f];
+          xyz_counts: int32 CUDA tensor (nframes, 2), ground and non-ground rows of every frame (None without an xyz part),
+            so frame f's non-ground cloud is nonground_xyz[row_off[f]:][:xyz_counts[f, 1]];
+          centers, normals: float32 CUDA tensors (nframes, patch_row_stride, 3), num_patches int32 [nframes]: frame f's patches
+            are centers[f, :num_patches[f]];
+          height (nframes,), elevation_thr, flatness_thr (nframes, 4) float64 and n_elevation, n_flatness (nframes, 4) int32:
+            strided CUDA views of the state rows (None when the state is not enabled), row f the state of frame f's stream
+            right after frame f."""
+        import torch
+        g = PwppBoundGetters()
+        _check(self.lib.pwpp_bound_getter_results(self._h, C.byref(g)))
+        nf = len(self._bound[0])
+        row_off = np.ctypeslib.as_array((C.c_int64 * (nf + 1)).from_address(g.h_row_off)).copy()
+        rows, stride = int(row_off[-1]), int(g.patch_row_stride)
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr, shape, typestr, strides=None):
+                self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (ptr, False), "version": 3, "strides": strides}
+
+        def view(ptr, shape, typestr, strides=None):
+            if not ptr:
+                return None
+            if 0 in shape:
+                return torch.empty(shape, dtype={"<f4": torch.float32, "<f8": torch.float64, "<i4": torch.int32}[typestr], device="cuda")
+            return torch.as_tensor(_View(ptr, shape, typestr, strides), device="cuda")
+        st = C.sizeof(PwppState)
+        s = g.states
+        return {"ground_xyz": view(g.ground_xyz, (rows, 3), "<f4"), "nonground_xyz": view(g.nonground_xyz, (rows, 3), "<f4"),
+                "row_off": row_off, "xyz_counts": view(g.xyz_counts, (nf, 2), "<i4"),
+                "centers": view(g.centers, (nf, stride, 3), "<f4"), "normals": view(g.normals, (nf, stride, 3), "<f4"),
+                "num_patches": view(g.num_patches, (nf,), "<i4"),
+                "height": view(s, (nf,), "<f8", (st,)),
+                "elevation_thr": view(s and s + PwppState.elevation_thr.offset, (nf, 4), "<f8", (st, 8)),
+                "flatness_thr": view(s and s + PwppState.flatness_thr.offset, (nf, 4), "<f8", (st, 8)),
+                "n_elevation": view(s and s + PwppState.n_elevation.offset, (nf, 4), "<i4", (st, 4)),
+                "n_flatness": view(s and s + PwppState.n_flatness.offset, (nf, 4), "<i4", (st, 4))}
 
     def unbind_call(self):
         _check(self.lib.pwpp_unbind_call(self._h))

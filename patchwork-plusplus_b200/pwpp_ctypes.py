@@ -56,3 +56,10 @@ class PwppPointLayout(C.Structure):
 class PwppScanRing(C.Structure):
     """Mirror of `pwpp_scan_ring` (include/pwpp.h): a ring of scan slots in device memory for pwpp_bind_call_rings."""
     _fields_ = [("base", C.c_void_p), ("slot_stride", C.c_int64), ("d_counts", C.c_void_p), ("num_slots", C.c_int32), ("_pad", C.c_int32)]
+
+
+class PwppBoundGetters(C.Structure):
+    """Mirror of `pwpp_bound_getters` (include/pwpp.h): the fixed device pointers of a bound call's getter results."""
+    _fields_ = [("ground_xyz", C.c_void_p), ("nonground_xyz", C.c_void_p), ("h_row_off", C.c_void_p), ("xyz_counts", C.c_void_p),
+                ("centers", C.c_void_p), ("normals", C.c_void_p), ("num_patches", C.c_void_p), ("patch_row_stride", C.c_int64),
+                ("states", C.c_void_p)]
