@@ -12,6 +12,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "pwpp.h"
@@ -54,11 +55,18 @@ int fail(int code, const std::string& msg) {
 
 unsigned long long g_alloc_gen = 0;   // bumped whenever a device buffer moves: captured CUDA graphs hold the old pointers
 
-// InGraphs = false: a buffer no captured launch sequence reads (its moves leave the graphs valid)
+// InGraphs = false: a buffer no captured launch sequence reads (its moves leave the graphs valid).
+// A buffer owns its allocation: it frees it when destroyed, and a move hands it over and leaves the source empty.
 template <typename T, bool InGraphs = true>
 struct DevBuf {
   T* p = nullptr;
   size_t cap = 0;  // elements
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); o.release(); return *this; }
+  ~DevBuf() { release(); }
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
     if (InGraphs) ++g_alloc_gen;
@@ -91,6 +99,12 @@ template <typename T>
 struct PinBuf {
   T* p = nullptr;
   size_t cap = 0;
+  PinBuf() = default;
+  PinBuf(const PinBuf&) = delete;
+  PinBuf& operator=(const PinBuf&) = delete;
+  PinBuf(PinBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  PinBuf& operator=(PinBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); o.release(); return *this; }
+  ~PinBuf() { release(); }
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
     if (p) cudaFreeHost(p);
@@ -225,7 +239,8 @@ struct pwpp_ctx {
   cudaStream_t last_stream = nullptr;
   bool last_bound = false, off_fetched = false;   // the last call is the bound call; its point offsets were fetched (fetch_offsets)
 
-  // the bound call (pwpp_bind_call): what its runs re-establish and launch. The work buffers are frozen while it is bound.
+  // the bound call (pwpp_bind_call): what its runs re-establish and launch, and the device buffers it owns (released with it).
+  // The work buffers are frozen while it is bound.
   struct Bound {
     bool on = false;
     int nf = 0, has_intensity = 0;
@@ -233,33 +248,33 @@ struct pwpp_ctx {
     long long unpack_gx = 0;                // grid.x of the unpack, from the capacities
     std::vector<int> runs, frame_set, run_chunks, cap_chunk_off;   // run_chunks[r]: the run's largest ceil(max_n / CHUNK_PTS)
     std::vector<long long> cap_pt_off;      // the capacity layout: sizes grids and picks the dense front end only
+    DevBuf<long long, false> d_bmax;        // [F] max_n
+    DevBuf<int, false> d_bstream, d_bpset;  // [F] the bound call's stream and set tables
+    DevBuf<int, false> d_bstatus;           // [F] PWPP_COUNT_OUT_OF_RANGE or 0
+    std::vector<RecordFrame> recs;          // its record table (host copy of d_brec)
+    DevBuf<RecordFrame, false> d_brec;      // [F] its record table
     int rec_parts = 0;                      // record results (pwpp_bind_record_results): PWPP_PART_* bits, 0 = off
     long long rec_gx = 0;                   // grid.x of k_gather_record_parts, from the capacities
-    std::vector<RecordFrame> recs;          // its record table (host copy of d_brec)
     std::vector<long long> rec_part_off;    // [F+1] byte offsets of every frame's region in each part buffer
+    DevBuf<unsigned char, false> d_bground, d_bnonground;   // its record results, one buffer per part (region f at rec_part_off[f])
+    DevBuf<long long, false> d_bpart_off;   // [F+1] rec_part_off
+    DevBuf<int, false> d_rec_counts;        // [F][2]: ground, non-ground records of every frame of the last run
     const int* d_actions = nullptr;         // the caller's device actions (pwpp_bind_call_actions), NULL: none
     std::vector<char> reset_run;            // [runs] the run holds a frame whose stream ran in an earlier run: k_bound_reset
+    DevBuf<int, false> d_bscratch, d_bdep;  // [F] with actions: scratch slot of every frame; its stream has a frame in an earlier run
+    DevBuf<int, false> d_bact;              // [F] the run's copy of the actions
     const int* d_slots = nullptr;           // the caller's device slots (pwpp_bind_call_rings), NULL: no rings
+    DevBuf<BoundRing, false> d_bring;       // [F] with rings: every frame's ring
+    DevBuf<int, false> d_bslot;             // [F] the run's copy of the slots
+    DevBuf<RecordFrame, false> d_brun;      // [F] the run's record table (d_brec with every frame's slot applied)
     int getters = 0;                        // getter results (pwpp_bind_getter_results): PWPP_GETTER_* bits, 0 = off
     long long xyz_gx = 0;                   // grid.x of k_gather_xyz_parts, from the capacities
+    DevBuf<float, false> d_bgxyz, d_bngxyz;  // getter results: [sum(max_n)][3] ground / non-ground xyz, frame f from row cap_pt_off[f]
+    DevBuf<long long, false> d_bxyz_off;    // [F+1] cap_pt_off
+    DevBuf<int, false> d_xyz_counts;        // [F][2]: ground, non-ground xyz rows of every frame of the last run
+    DevBuf<pwpp_state, false> d_bstates;    // [F] the state of every frame's stream right after the frame
   } bound;
   int scratch_slots = 0;                  // state / history slots after the streams' (pwpp_bind_call_actions), kept after unbind
-  DevBuf<long long, false> d_bmax;        // [F] max_n
-  DevBuf<int, false> d_bstream, d_bpset;  // [F] the bound call's stream and set tables
-  DevBuf<int, false> d_bstatus;           // [F] PWPP_COUNT_OUT_OF_RANGE or 0
-  DevBuf<RecordFrame, false> d_brec;      // [F] its record table
-  DevBuf<unsigned char, false> d_bground, d_bnonground;   // its record results, one buffer per part (region f at rec_part_off[f])
-  DevBuf<long long, false> d_bpart_off;   // [F+1] rec_part_off
-  DevBuf<int, false> d_rec_counts;        // [F][2]: ground, non-ground records of every frame of the last run
-  DevBuf<int, false> d_bscratch, d_bdep;  // [F] with actions: scratch slot of every frame; its stream has a frame in an earlier run
-  DevBuf<int, false> d_bact;              // [F] the run's copy of the actions
-  DevBuf<BoundRing, false> d_bring;       // [F] with rings: every frame's ring
-  DevBuf<int, false> d_bslot;             // [F] the run's copy of the slots
-  DevBuf<RecordFrame, false> d_brun;      // [F] the run's record table (d_brec with every frame's slot applied)
-  DevBuf<float, false> d_bgxyz, d_bngxyz;  // getter results: [sum(max_n)][3] ground / non-ground xyz, frame f from row cap_pt_off[f]
-  DevBuf<long long, false> d_bxyz_off;    // [F+1] cap_pt_off
-  DevBuf<int, false> d_xyz_counts;        // [F][2]: ground, non-ground xyz rows of every frame of the last run
-  DevBuf<pwpp_state, false> d_bstates;    // [F] the state of every frame's stream right after the frame
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
   struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
@@ -267,6 +282,9 @@ struct pwpp_ctx {
   GraphKey gkey[2] = {};
   long long glaunches[2] = {0, 0};
   int sw_graph = 1;
+
+  // frees every buffer (pwpp_destroy); not exported: the context is opaque to callers
+  __attribute__((visibility("hidden"))) ~pwpp_ctx() = default;
 };
 
 namespace {
@@ -702,6 +720,110 @@ int run_path(pwpp_ctx* ctx, int nframes, const int32_t* streams, const float4* d
   return launch_call(ctx, nframes, d_pts, has_intensity, s);
 }
 
+// A page-locked host buffer, which the upload can read by DMA straight from.
+bool page_locked(const void* p) {
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, p) == cudaSuccess) return attr.type == cudaMemoryTypeHost;
+  cudaGetLastError();
+  return false;
+}
+
+// The host-input pipeline of pwpp_estimate_host(_streams) and pwpp_estimate_host_records, after their argument checks, from
+// the freeze check to last_time_us. Chunks of frames flow through three streams: H2D of chunk k+1 | kernels of chunk k | D2H
+// of chunk k-1. The caller supplies only what is its own: tables(&recs) reserves and fills its tables once the previous call
+// is no longer in flight, before the call is prepared, and names its record table (NULL: none); stage(f0, f1, s_in) puts
+// frames [f0, f1) into ctx->d_in on the upload stream s_in.
+template <typename Tables, typename Stage>
+int host_pipeline(pwpp_ctx* ctx, int nframes, const int32_t* streams, const int64_t* n, int has_intensity, Tables tables, Stage stage) {
+  int rc = check_frozen(ctx, nframes, n, true);
+  if (rc) return rc;
+  rc = bind_device(ctx);
+  if (rc) return rc;
+  const auto t0 = std::chrono::steady_clock::now();
+  ctx->pt_off.assign(nframes + 1, 0);
+  for (int f = 0; f < nframes; ++f) ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
+  const long long total = ctx->pt_off[nframes];
+  cudaStream_t s = ctx->stream, s_in = ctx->stream_h2d, s_out = ctx->stream_d2h;
+  ctx->call_times_valid = false;
+  // the staging buffers of the previous call must not be in flight any more (nor a device-input call on a caller's stream)
+  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  CU_TRY(cudaStreamSynchronize(s));
+  CU_TRY(cudaStreamSynchronize(s_in));
+  CU_TRY(cudaStreamSynchronize(s_out));
+  CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(total, 1)));
+  const RecordFrame* recs = nullptr;
+  rc = tables(&recs);
+  if (rc) return rc;
+  rc = prepare_call(ctx, nframes, streams, s, recs);
+  if (rc) return rc;
+  CU_TRY(ctx->h_out_idx.reserve((size_t) std::max<long long>(total, 1)));
+  CU_TRY(ctx->h_counts.reserve((size_t) 3 * nframes));
+  // ~64 MB of points per chunk keeps every stage busy without delaying the first kernels
+  int chunk_frames = nframes;
+  if (nframes > 1 && total > 0) {
+    const long long per_frame = std::max<long long>(1, total / nframes);
+    chunk_frames = (int) std::min<long long>(nframes, std::max<long long>(1, (4LL << 20) / per_frame));
+  }
+  const int nchunks = (nframes + chunk_frames - 1) / chunk_frames;
+  // a call that is a single chunk has nothing to pipeline: copies and kernels share one stream (no cross-stream event hops
+  // on the critical path of a one-frame call) and four events bracket its three phases (pwpp_call_times_us)
+  const bool one_stream = (nchunks == 1);
+  if (one_stream) { s_in = s; s_out = s; CU_TRY(cudaEventRecord(ctx->ev_begin, s)); }
+  // the launch ranges are the pipeline chunks cut at the run boundaries; per-stage timing needs one range per call
+  const bool prof = ctx->profiling && nchunks == 1 && ctx->runs.size() == 2;
+  size_t run_cursor = 0;
+  for (int k = 0; k < nchunks; ++k) {
+    const int f0 = k * chunk_frames, f1 = std::min(nframes, f0 + chunk_frames);
+    rc = stage(f0, f1, s_in);
+    if (rc) return rc;
+    CU_TRY(cudaEventRecord(ctx->ev0, s_in));
+    if (!one_stream) CU_TRY(cudaStreamWaitEvent(s, ctx->ev0, 0));
+    rc = launch_runs(ctx, f0, f1, &run_cursor, ctx->d_in.p, has_intensity, s, prof);
+    if (rc) return rc;
+    CU_TRY(cudaEventRecord(ctx->ev1, s));
+    if (!one_stream) CU_TRY(cudaStreamWaitEvent(s_out, ctx->ev1, 0));
+    const long long o0 = ctx->pt_off[f0], o1 = ctx->pt_off[f1];
+    if (f0 == 0 && f1 == nframes) {   // the three count rows are one contiguous block when the chunk covers the whole call
+      CU_TRY(cudaMemcpyAsync(ctx->h_counts.p, ctx->d_counts.p, (size_t) 3 * nframes * sizeof(int), cudaMemcpyDeviceToHost, s_out));
+    } else {
+      for (int q = 0; q < 3; ++q)
+        CU_TRY(cudaMemcpyAsync(ctx->h_counts.p + (size_t) q * nframes + f0, ctx->d_counts.p + (size_t) q * nframes + f0,
+                               (size_t) (f1 - f0) * sizeof(int), cudaMemcpyDeviceToHost, s_out));
+    }
+    if (o1 > o0) CU_TRY(cudaMemcpyAsync(ctx->h_out_idx.p + o0, ctx->d_out_idx.p + o0, (size_t) (o1 - o0) * sizeof(int), cudaMemcpyDeviceToHost, s_out));
+  }
+  if (one_stream) CU_TRY(cudaEventRecord(ctx->ev_end, s));
+  CU_TRY(cudaStreamSynchronize(s_out));
+  CU_TRY(cudaStreamSynchronize(s));
+  ctx->call_times_valid = one_stream;
+  ctx->counts_fetched = true;
+  ctx->idx_fetched = true;
+  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
+  return PWPP_OK;
+}
+
+// The device-input calls after their argument checks: the freeze check of frames of n[f] points, the frame offsets
+// (ctx->pt_off), the stream order and, with_input, the ctx's input buffer; body(s) then enqueues the call on its stream s.
+template <typename Body>
+int device_call(pwpp_ctx* ctx, int nframes, const int64_t* n, bool with_input, void* cuda_stream, Body body) {
+  int rc = check_frozen(ctx, nframes, n, with_input);
+  if (rc) return rc;
+  rc = bind_device(ctx);
+  if (rc) return rc;
+  const auto t0 = std::chrono::steady_clock::now();
+  ctx->pt_off.assign(nframes + 1, 0);
+  for (int f = 0; f < nframes; ++f) ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
+  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
+  // work buffers are reused stream-ordered: a call on a different stream than the previous one waits for it
+  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  if (!ctx->last_stream && s != ctx->stream) CU_TRY(cudaStreamSynchronize(ctx->stream));   // resets issued before the first call ran on the ctx's own stream
+  if (with_input) CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(ctx->pt_off[nframes], 1)));
+  rc = body(s);
+  if (rc) return rc;
+  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
+  return PWPP_OK;
+}
+
 int check_frame(pwpp_ctx* ctx, int f) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (f < 0 || f >= ctx->last_nframes) return fail(PWPP_ERR_INVALID_ARG, "frame index outside the last estimate call");
@@ -762,6 +884,13 @@ int fetch_patches(pwpp_ctx* ctx) {
 inline int frame_n(const pwpp_ctx* ctx, int f) { return (int) (ctx->pt_off[f + 1] - ctx->pt_off[f]); }
 // fetched count of frame f: q = 0 ground points, 1 patches, 2 dropped points
 inline int count_of(const pwpp_ctx* ctx, int q, int f) { return ctx->h_counts.p[(size_t) q * ctx->last_nframes + f]; }
+// frame f's ground or non-ground list in the fetched counts: its start inside the frame's region (the non-ground list follows
+// the ground list) and its length (the dropped points are in neither)
+struct FrameList { int start, count; };
+inline FrameList frame_list(const pwpp_ctx* ctx, int f, bool ground) {
+  const int ng = count_of(ctx, 0, f);
+  return ground ? FrameList{0, ng} : FrameList{ng, frame_n(ctx, f) - ng - count_of(ctx, 2, f)};
+}
 
 }  // namespace
 
@@ -993,24 +1122,7 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
   for (int i = 0; i < 2; ++i) if (ctx->tab_ev[i]) cudaEventDestroy(ctx->tab_ev[i]);
   for (int q = 0; q < NUM_SIDE; ++q) { if (ctx->ev_fit[q]) cudaEventDestroy(ctx->ev_fit[q]); if (ctx->ev_join[q]) cudaEventDestroy(ctx->ev_join[q]); if (ctx->side[q]) cudaStreamDestroy(ctx->side[q]); }
-  ctx->d_states.release(); ctx->d_states_init.release(); ctx->d_hist.release(); ctx->d_in.release(); ctx->d_cm.release(); ctx->d_pt_off.release(); ctx->d_chunk_off.release();
-  ctx->d_stream.release(); ctx->d_pset.release();
-  ctx->d_bin_ids.release(); ctx->d_chist.release(); ctx->d_cbase.release(); ctx->d_bin_off.release(); ctx->d_sorted.release();
-  ctx->d_part.release(); ctx->d_labels.release(); ctx->d_fits.release(); ctx->d_segs.release(); ctx->d_wq_ctr.release();
-  for (int c = 0; c < NUM_CLASSES; ++c) ctx->d_wq_items[c].release();
-  ctx->d_out_idx.release(); ctx->d_counts.release();
-  ctx->d_centers.release(); ctx->d_normals.release(); ctx->d_xyz.release();
-  ctx->d_raw.release(); ctx->d_rec.release(); ctx->h_raw.release(); for (int i = 0; i < 2; ++i) ctx->h_rec_buf[i].release();
-  ctx->d_rec_out.release(); ctx->d_rec_off.release(); ctx->h_rec_off.release(); ctx->h_rec_out.release();
-  ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
-  ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
-  ctx->d_bscratch.release(); ctx->d_bdep.release(); ctx->d_bact.release();
-  ctx->d_bring.release(); ctx->d_bslot.release(); ctx->d_brun.release();
-  ctx->d_bgxyz.release(); ctx->d_bngxyz.release(); ctx->d_bxyz_off.release(); ctx->d_xyz_counts.release(); ctx->d_bstates.release();
   if (ctx->ev_rec_off) cudaEventDestroy(ctx->ev_rec_off);
-  ctx->h_in.release(); for (int i = 0; i < 2; ++i) { ctx->h_pt_off_buf[i].release(); ctx->h_chunk_off_buf[i].release(); ctx->h_stream_buf[i].release(); ctx->h_pset_buf[i].release(); }
-  ctx->h_out_idx.release(); ctx->h_counts.release();
-  ctx->h_centers.release(); ctx->h_normals.release();
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
   if (ctx->ev_begin) cudaEventDestroy(ctx->ev_begin);
@@ -1018,7 +1130,7 @@ void pwpp_destroy(pwpp_ctx* ctx) {
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   if (ctx->stream_h2d) cudaStreamDestroy(ctx->stream_h2d);
   if (ctx->stream_d2h) cudaStreamDestroy(ctx->stream_d2h);
-  delete ctx;
+  delete ctx;   // the buffers free themselves, on the device set above
 }
 
 int pwpp_reset_stream(pwpp_ctx* ctx, int f) {
@@ -1073,55 +1185,15 @@ static int estimate_host_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams
   if (cols != 3 && cols != 4) return fail(PWPP_ERR_INVALID_ARG, "cols must be 3 or 4 (x,y,z[,intensity])");
   for (int f = 0; f < nframes; ++f)
     if (n[f] < 0 || (n[f] > 0 && !pts[f])) return fail(PWPP_ERR_INVALID_ARG, "bad frame pointer/size");
-  int rc = check_frozen(ctx, nframes, n, true);
-  if (rc) return rc;
-  rc = bind_device(ctx);
-  if (rc) return rc;
-  const auto t0 = std::chrono::steady_clock::now();
-  ctx->pt_off.assign(nframes + 1, 0);
-  for (int f = 0; f < nframes; ++f) ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
-  const long long total = ctx->pt_off[nframes];
-  CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(total, 1)));
-  cudaStream_t s = ctx->stream, s_in = ctx->stream_h2d, s_out = ctx->stream_d2h;
-  ctx->call_times_valid = false;
-  // the staging buffers of the previous call must not be in flight any more (nor a device-input call on a caller's stream)
-  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
-  CU_TRY(cudaStreamSynchronize(s));
-  CU_TRY(cudaStreamSynchronize(s_in));
-  CU_TRY(cudaStreamSynchronize(s_out));
-  rc = prepare_call(ctx, nframes, streams, s);
-  if (rc) return rc;
-  CU_TRY(ctx->h_out_idx.reserve((size_t) std::max<long long>(total, 1)));
-  CU_TRY(ctx->h_counts.reserve((size_t) 3 * nframes));
   const bool packed = (cols == 4 && col_stride == 1 && row_stride == 4);
   bool staged_any = false;
-  // Chunks of frames flow through three streams: H2D of chunk k+1 | kernels of chunk k | D2H of chunk k-1.
-  // ~64 MB of points per chunk keeps every stage busy without delaying the first kernels.
-  int chunk_frames = nframes;
-  if (nframes > 1 && total > 0) {
-    const long long per_frame = std::max<long long>(1, total / nframes);
-    chunk_frames = (int) std::min<long long>(nframes, std::max<long long>(1, (4LL << 20) / per_frame));
-  }
-  const int nchunks = (nframes + chunk_frames - 1) / chunk_frames;
-  // a call that is a single chunk has nothing to pipeline: copies and kernels share one stream (no cross-stream event hops
-  // on the critical path of a one-frame call) and four events bracket its three phases (pwpp_call_times_us)
-  const bool one_stream = (nchunks == 1);
-  if (one_stream) { s_in = s; s_out = s; CU_TRY(cudaEventRecord(ctx->ev_begin, s)); }
-  // the launch ranges are the pipeline chunks cut at the run boundaries; per-stage timing needs one range per call
-  const bool prof = ctx->profiling && nchunks == 1 && ctx->runs.size() == 2;
-  size_t run_cursor = 0;
-  for (int k = 0; k < nchunks; ++k) {
-    const int f0 = k * chunk_frames, f1 = std::min(nframes, f0 + chunk_frames);
+  auto no_tables = [](const RecordFrame**) -> int { return PWPP_OK; };
+  auto stage = [&](int f0, int f1, cudaStream_t s_in) -> int {
+    const long long total = ctx->pt_off[nframes];
     for (int f = f0; f < f1; ++f) {
       const int64_t cnt = n[f];
       if (cnt == 0) continue;
-      bool pinned = false;
-      if (packed) {
-        cudaPointerAttributes attr;
-        if (cudaPointerGetAttributes(&attr, pts[f]) == cudaSuccess) pinned = (attr.type == cudaMemoryTypeHost);
-        else cudaGetLastError();
-      }
-      if (pinned) {  // page-locked caller buffer: DMA straight from it (the private copy of H:152 is the device buffer)
+      if (packed && page_locked(pts[f])) {  // page-locked caller buffer: DMA straight from it (the private copy of H:152 is the device buffer)
         // frames that follow each other in the caller's buffer travel as one copy
         int f_last = f;
         int64_t run = cnt;
@@ -1153,30 +1225,9 @@ static int estimate_host_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams
       }
       CU_TRY(cudaMemcpyAsync(ctx->d_in.p + ctx->pt_off[f], dst, (size_t) cnt * sizeof(float4), cudaMemcpyHostToDevice, s_in));
     }
-    CU_TRY(cudaEventRecord(ctx->ev0, s_in));
-    if (!one_stream) CU_TRY(cudaStreamWaitEvent(s, ctx->ev0, 0));
-    rc = launch_runs(ctx, f0, f1, &run_cursor, ctx->d_in.p, cols == 4 ? 1 : 0, s, prof);
-    if (rc) return rc;
-    CU_TRY(cudaEventRecord(ctx->ev1, s));
-    if (!one_stream) CU_TRY(cudaStreamWaitEvent(s_out, ctx->ev1, 0));
-    const long long o0 = ctx->pt_off[f0], o1 = ctx->pt_off[f1];
-    if (f0 == 0 && f1 == nframes) {   // the three count rows are one contiguous block when the chunk covers the whole call
-      CU_TRY(cudaMemcpyAsync(ctx->h_counts.p, ctx->d_counts.p, (size_t) 3 * nframes * sizeof(int), cudaMemcpyDeviceToHost, s_out));
-    } else {
-      for (int q = 0; q < 3; ++q)
-        CU_TRY(cudaMemcpyAsync(ctx->h_counts.p + (size_t) q * nframes + f0, ctx->d_counts.p + (size_t) q * nframes + f0,
-                               (size_t) (f1 - f0) * sizeof(int), cudaMemcpyDeviceToHost, s_out));
-    }
-    if (o1 > o0) CU_TRY(cudaMemcpyAsync(ctx->h_out_idx.p + o0, ctx->d_out_idx.p + o0, (size_t) (o1 - o0) * sizeof(int), cudaMemcpyDeviceToHost, s_out));
-  }
-  if (one_stream) CU_TRY(cudaEventRecord(ctx->ev_end, s));
-  CU_TRY(cudaStreamSynchronize(s_out));
-  CU_TRY(cudaStreamSynchronize(s));
-  ctx->call_times_valid = one_stream;
-  ctx->counts_fetched = true;
-  ctx->idx_fetched = true;
-  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
-  return PWPP_OK;
+    return PWPP_OK;
+  };
+  return host_pipeline(ctx, nframes, streams, n, cols == 4 ? 1 : 0, no_tables, stage);
 }
 
 int pwpp_estimate_host(pwpp_ctx* ctx, int nframes, const float* const* pts, const int64_t* n, int cols, int64_t row_stride, int64_t col_stride) {
@@ -1193,33 +1244,26 @@ int pwpp_estimate_host_streams(pwpp_ctx* ctx, int nframes, const int32_t* stream
   return estimate_host_impl(ctx, nframes, streams, pts, n, cols, row_stride, col_stride);
 }
 
+// The frame sizes of a device-input call's offsets, which must be non-decreasing.
+static int offset_sizes(int nframes, const int64_t* h_offsets, int64_t* sizes) {
+  for (int f = 0; f < nframes; ++f) {
+    sizes[f] = h_offsets[f + 1] - h_offsets[f];
+    if (sizes[f] < 0) return fail(PWPP_ERR_INVALID_ARG, "offsets must be non-decreasing");
+  }
+  return PWPP_OK;
+}
+
 // The device path of pwpp_estimate_device and pwpp_estimate_device_streams (stream table checked by the caller).
 static int estimate_device_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* d_pts, const int64_t* h_offsets, int has_intensity,
                                 void* cuda_stream) {
   if (!h_offsets) return fail(PWPP_ERR_INVALID_ARG, "NULL argument");
-  for (int f = 1; f <= nframes; ++f)
-    if (h_offsets[f] < h_offsets[f - 1]) return fail(PWPP_ERR_INVALID_ARG, "offsets must be non-decreasing");
+  std::vector<int64_t> sizes(nframes);
+  int rc = offset_sizes(nframes, h_offsets, sizes.data());
+  if (rc) return rc;
   if (h_offsets[nframes] > h_offsets[0] && !d_pts) return fail(PWPP_ERR_INVALID_ARG, "d_pts is NULL");
-  int rc = PWPP_OK;
-  if (ctx->bound.on) {
-    std::vector<int64_t> sizes(nframes);
-    for (int f = 0; f < nframes; ++f) sizes[f] = h_offsets[f + 1] - h_offsets[f];
-    rc = check_frozen(ctx, nframes, sizes.data(), false);
-    if (rc) return rc;
-  }
-  rc = bind_device(ctx);
-  if (rc) return rc;
-  const auto t0 = std::chrono::steady_clock::now();
-  ctx->pt_off.assign(nframes + 1, 0);
-  for (int f = 0; f <= nframes; ++f) ctx->pt_off[f] = h_offsets[f] - h_offsets[0];
-  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
-  // work buffers are reused stream-ordered: a call on a different stream than the previous one waits for it
-  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
-  if (!ctx->last_stream && s != ctx->stream) CU_TRY(cudaStreamSynchronize(ctx->stream));   // resets issued before the first call ran on the ctx's own stream
-  rc = run_path(ctx, nframes, streams, (const float4*) d_pts + h_offsets[0], has_intensity, s);
-  if (rc) return rc;
-  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
-  return PWPP_OK;
+  return device_call(ctx, nframes, sizes.data(), false, cuda_stream, [&](cudaStream_t s) {
+    return run_path(ctx, nframes, streams, (const float4*) d_pts + h_offsets[0], has_intensity, s);
+  });
 }
 
 int pwpp_estimate_device(pwpp_ctx* ctx, int nframes, const void* d_pts, const int64_t* h_offsets, int has_intensity, void* cuda_stream) {
@@ -1239,27 +1283,18 @@ int pwpp_estimate_device_streams(pwpp_ctx* ctx, int nframes, const int32_t* stre
 int pwpp_estimate_device_xyz(pwpp_ctx* ctx, int nframes, const void* d_xyz, const int64_t* h_offsets, void* cuda_stream) {
   if (!ctx || !h_offsets) return fail(PWPP_ERR_INVALID_ARG, "NULL argument");
   if (nframes < 1 || nframes > ctx->num_streams) return fail(PWPP_ERR_INVALID_ARG, "nframes must be in [1, num_streams]");
-  int rc = bind_device(ctx);
-  if (rc) return rc;
   const long long total = h_offsets[nframes] - h_offsets[0];
   if (total < 0 || (total > 0 && !d_xyz)) return fail(PWPP_ERR_INVALID_ARG, "bad offsets / d_xyz is NULL");
-  if (ctx->bound.on) {
-    std::vector<int64_t> sizes(nframes);
-    for (int f = 0; f < nframes; ++f) sizes[f] = h_offsets[f + 1] - h_offsets[f];
-    rc = check_frozen(ctx, nframes, sizes.data(), true);
-    if (rc) return rc;
-  }
-  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
-  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
-  if (!ctx->last_stream && s != ctx->stream) CU_TRY(cudaStreamSynchronize(ctx->stream));
-  CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(total, 1)));
-  if (total > 0) {
-    k_pad_xyz<<<(unsigned) ((total + 255) / 256), 256, 0, s>>>((const float*) d_xyz + 3 * h_offsets[0], total, ctx->d_in.p);
-    ++ctx->launches;
-  }
-  std::vector<int64_t> offs(h_offsets, h_offsets + nframes + 1);
-  for (auto& o : offs) o -= h_offsets[0];
-  return pwpp_estimate_device(ctx, nframes, ctx->d_in.p, offs.data(), 0, s);
+  std::vector<int64_t> sizes(nframes);
+  const int rc = offset_sizes(nframes, h_offsets, sizes.data());
+  if (rc) return rc;
+  return device_call(ctx, nframes, sizes.data(), true, cuda_stream, [&](cudaStream_t s) {
+    if (total > 0) {
+      k_pad_xyz<<<(unsigned) ((total + 255) / 256), 256, 0, s>>>((const float*) d_xyz + 3 * h_offsets[0], total, ctx->d_in.p);
+      ++ctx->launches;
+    }
+    return run_path(ctx, nframes, ctx->identity.data(), ctx->d_in.p, 0, s);
+  });
 }
 
 // The checks of both records entry points (include/pwpp.h), before anything is allocated or launched.
@@ -1276,14 +1311,6 @@ static int check_records_call(pwpp_ctx* ctx, int nframes, const int32_t* streams
   return PWPP_OK;
 }
 
-// The checks of a direct records call: those above, and the freeze of a bound call.
-static int check_direct_records_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* n,
-                                     const pwpp_point_layout* layouts) {
-  const int rc = check_records_call(ctx, nframes, streams, frames, n, layouts);
-  if (rc) return rc;
-  return check_frozen(ctx, nframes, n, true);
-}
-
 // Unpacks frames [f0, f1) of the prepared records call into ctx->d_in on stream s: one launch (none when the frames are empty).
 static int unpack_records(pwpp_ctx* ctx, int f0, int f1, const std::vector<RecordFrame>& recs, cudaStream_t s) {
   if (ctx->pt_off[f1] == ctx->pt_off[f0]) return PWPP_OK;
@@ -1296,120 +1323,59 @@ static int unpack_records(pwpp_ctx* ctx, int f0, int f1, const std::vector<Recor
 
 int pwpp_estimate_host_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* n,
                                const pwpp_point_layout* layouts) {
-  int rc = check_direct_records_call(ctx, nframes, streams, frames, n, layouts);
+  const int rc = check_records_call(ctx, nframes, streams, frames, n, layouts);
   if (rc) return rc;
-  rc = bind_device(ctx);
-  if (rc) return rc;
-  const auto t0 = std::chrono::steady_clock::now();
-  ctx->pt_off.assign(nframes + 1, 0);
   std::vector<long long> raw_off(nframes + 1, 0);   // every frame's records in the upload buffer, 16-byte aligned
-  for (int f = 0; f < nframes; ++f) {
-    ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
-    raw_off[f + 1] = raw_off[f] + ((n[f] * layouts[f].point_step + 15) & ~15LL);
-  }
-  const long long total = ctx->pt_off[nframes];
-  cudaStream_t s = ctx->stream, s_in = ctx->stream_h2d, s_out = ctx->stream_d2h;
-  ctx->call_times_valid = false;
-  // the buffers of the previous call must not be in flight any more (nor a device-input call on a caller's stream)
-  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
-  CU_TRY(cudaStreamSynchronize(s));
-  CU_TRY(cudaStreamSynchronize(s_in));
-  CU_TRY(cudaStreamSynchronize(s_out));
-  CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(total, 1)));
-  CU_TRY(ctx->d_raw.reserve((size_t) std::max<long long>(raw_off[nframes], 16)));
-  std::vector<RecordFrame> recs(nframes);
   int has_intensity = 0;
   for (int f = 0; f < nframes; ++f) {
-    recs[f] = record_frame(layouts[f], ctx->d_raw.p + raw_off[f]);
+    raw_off[f + 1] = raw_off[f] + ((n[f] * layouts[f].point_step + 15) & ~15LL);
     if (layouts[f].offset[3] >= 0) has_intensity = 1;
   }
-  rc = prepare_call(ctx, nframes, streams, s, recs.data());
-  if (rc) return rc;
-  CU_TRY(ctx->h_out_idx.reserve((size_t) std::max<long long>(total, 1)));
-  CU_TRY(ctx->h_counts.reserve((size_t) 3 * nframes));
+  std::vector<RecordFrame> recs(nframes);
+  auto tables = [&](const RecordFrame** out) -> int {
+    CU_TRY(ctx->d_raw.reserve((size_t) std::max<long long>(raw_off[nframes], 16)));
+    for (int f = 0; f < nframes; ++f) recs[f] = record_frame(layouts[f], ctx->d_raw.p + raw_off[f]);
+    *out = recs.data();
+    return PWPP_OK;
+  };
   bool staged_any = false;
-  // the chunk pipeline of pwpp_estimate_host: H2D + unpack of chunk k+1 | kernels of chunk k | D2H of chunk k-1
-  int chunk_frames = nframes;
-  if (nframes > 1 && total > 0) {
-    const long long per_frame = std::max<long long>(1, total / nframes);
-    chunk_frames = (int) std::min<long long>(nframes, std::max<long long>(1, (4LL << 20) / per_frame));
-  }
-  const int nchunks = (nframes + chunk_frames - 1) / chunk_frames;
-  const bool one_stream = (nchunks == 1);
-  if (one_stream) { s_in = s; s_out = s; CU_TRY(cudaEventRecord(ctx->ev_begin, s)); }
-  else CU_TRY(cudaStreamWaitEvent(s_in, ctx->tab_ev[ctx->tab_cur], 0));   // the unpack reads the record table uploaded on s
-  const bool prof = ctx->profiling && nchunks == 1 && ctx->runs.size() == 2;
-  size_t run_cursor = 0;
-  for (int k = 0; k < nchunks; ++k) {
-    const int f0 = k * chunk_frames, f1 = std::min(nframes, f0 + chunk_frames);
+  // H2D + unpack of a chunk's records
+  auto stage = [&](int f0, int f1, cudaStream_t s_in) -> int {
+    // a call of several chunks unpacks on the upload stream, and the unpack reads the record table uploaded on the call's stream
+    if (f0 == 0 && s_in != ctx->stream) CU_TRY(cudaStreamWaitEvent(s_in, ctx->tab_ev[ctx->tab_cur], 0));
     for (int f = f0; f < f1; ++f) {
       if (n[f] == 0) continue;
       const size_t bytes = (size_t) n[f] * layouts[f].point_step;
-      bool pinned = false;
-      cudaPointerAttributes attr;
-      if (cudaPointerGetAttributes(&attr, frames[f]) == cudaSuccess) pinned = (attr.type == cudaMemoryTypeHost);
-      else cudaGetLastError();
       const void* src = frames[f];
-      if (!pinned) {   // pageable: one memcpy into page-locked staging, then DMA
+      if (!page_locked(src)) {   // pageable: one memcpy into page-locked staging, then DMA
         if (!staged_any) { CU_TRY(ctx->h_raw.reserve((size_t) std::max<long long>(raw_off[nframes], 16))); staged_any = true; }
         std::memcpy(ctx->h_raw.p + raw_off[f], frames[f], bytes);
         src = ctx->h_raw.p + raw_off[f];
       }
       CU_TRY(cudaMemcpyAsync(ctx->d_raw.p + raw_off[f], src, bytes, cudaMemcpyHostToDevice, s_in));
     }
-    rc = unpack_records(ctx, f0, f1, recs, s_in);
-    if (rc) return rc;
-    CU_TRY(cudaEventRecord(ctx->ev0, s_in));
-    if (!one_stream) CU_TRY(cudaStreamWaitEvent(s, ctx->ev0, 0));
-    rc = launch_runs(ctx, f0, f1, &run_cursor, ctx->d_in.p, has_intensity, s, prof);
-    if (rc) return rc;
-    CU_TRY(cudaEventRecord(ctx->ev1, s));
-    if (!one_stream) CU_TRY(cudaStreamWaitEvent(s_out, ctx->ev1, 0));
-    const long long o0 = ctx->pt_off[f0], o1 = ctx->pt_off[f1];
-    for (int q = 0; q < 3; ++q)
-      CU_TRY(cudaMemcpyAsync(ctx->h_counts.p + (size_t) q * nframes + f0, ctx->d_counts.p + (size_t) q * nframes + f0, (size_t) (f1 - f0) * sizeof(int),
-                             cudaMemcpyDeviceToHost, s_out));
-    if (o1 > o0) CU_TRY(cudaMemcpyAsync(ctx->h_out_idx.p + o0, ctx->d_out_idx.p + o0, (size_t) (o1 - o0) * sizeof(int), cudaMemcpyDeviceToHost, s_out));
-  }
-  if (one_stream) CU_TRY(cudaEventRecord(ctx->ev_end, s));
-  CU_TRY(cudaStreamSynchronize(s_out));
-  CU_TRY(cudaStreamSynchronize(s));
-  ctx->call_times_valid = one_stream;
-  ctx->counts_fetched = true;
-  ctx->idx_fetched = true;
-  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
-  return PWPP_OK;
+    return unpack_records(ctx, f0, f1, recs, s_in);
+  };
+  return host_pipeline(ctx, nframes, streams, n, has_intensity, tables, stage);
 }
 
 int pwpp_estimate_device_records(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* d_frames, const int64_t* n,
                                  const pwpp_point_layout* layouts, void* cuda_stream) {
-  int rc = check_direct_records_call(ctx, nframes, streams, d_frames, n, layouts);
+  const int rc = check_records_call(ctx, nframes, streams, d_frames, n, layouts);
   if (rc) return rc;
-  rc = bind_device(ctx);
-  if (rc) return rc;
-  const auto t0 = std::chrono::steady_clock::now();
-  ctx->pt_off.assign(nframes + 1, 0);
-  for (int f = 0; f < nframes; ++f) ctx->pt_off[f + 1] = ctx->pt_off[f] + n[f];
-  const long long total = ctx->pt_off[nframes];
-  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
-  // stream ordering of pwpp_estimate_device_xyz: the input buffer and work buffers are reused in stream order
-  if (ctx->last_stream && ctx->last_stream != s) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
-  if (!ctx->last_stream && s != ctx->stream) CU_TRY(cudaStreamSynchronize(ctx->stream));
-  CU_TRY(ctx->d_in.reserve((size_t) std::max<long long>(total, 1)));
-  std::vector<RecordFrame> recs(nframes);
-  int has_intensity = 0;
-  for (int f = 0; f < nframes; ++f) {
-    recs[f] = record_frame(layouts[f], d_frames[f]);
-    if (layouts[f].offset[3] >= 0) has_intensity = 1;
-  }
-  rc = prepare_call(ctx, nframes, streams, s, recs.data());
-  if (rc) return rc;
-  rc = unpack_records(ctx, 0, nframes, recs, s);
-  if (rc) return rc;
-  rc = launch_call(ctx, nframes, ctx->d_in.p, has_intensity, s);
-  if (rc) return rc;
-  ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
-  return PWPP_OK;
+  return device_call(ctx, nframes, n, true, cuda_stream, [&](cudaStream_t s) {
+    std::vector<RecordFrame> recs(nframes);
+    int has_intensity = 0;
+    for (int f = 0; f < nframes; ++f) {
+      recs[f] = record_frame(layouts[f], d_frames[f]);
+      if (layouts[f].offset[3] >= 0) has_intensity = 1;
+    }
+    int rc = prepare_call(ctx, nframes, streams, s, recs.data());
+    if (rc) return rc;
+    rc = unpack_records(ctx, 0, nframes, recs, s);
+    if (rc) return rc;
+    return launch_call(ctx, nframes, ctx->d_in.p, has_intensity, s);
+  });
 }
 
 // ---- the bound call (include/pwpp.h) ----
@@ -1535,34 +1501,35 @@ static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
   }
   rc = reserve_work(ctx, nframes, b.cap_pt_off[nframes], chunks, true, false);
   if (rc) return rc;
+  // the bound call's own buffers: an error from here on frees them with b
   if (d_actions) {
-    CU_TRY(ctx->d_bscratch.reserve(nframes));
-    CU_TRY(ctx->d_bdep.reserve(nframes));
-    CU_TRY(ctx->d_bact.reserve(nframes));
-    CU_TRY(cudaMemcpy(ctx->d_bscratch.p, scratch.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemcpy(ctx->d_bdep.p, dep.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemset(ctx->d_bact.p, 0, (size_t) nframes * sizeof(int)));
+    CU_TRY(b.d_bscratch.reserve(nframes));
+    CU_TRY(b.d_bdep.reserve(nframes));
+    CU_TRY(b.d_bact.reserve(nframes));
+    CU_TRY(cudaMemcpy(b.d_bscratch.p, scratch.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemcpy(b.d_bdep.p, dep.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemset(b.d_bact.p, 0, (size_t) nframes * sizeof(int)));
   }
-  CU_TRY(ctx->d_bmax.reserve(nframes));
-  CU_TRY(ctx->d_bstream.reserve(nframes));
-  CU_TRY(ctx->d_bpset.reserve(nframes));
-  CU_TRY(ctx->d_bstatus.reserve(nframes));
-  CU_TRY(ctx->d_brec.reserve(nframes));
-  CU_TRY(cudaMemcpy(ctx->d_bmax.p, max_n, (size_t) nframes * sizeof(long long), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(ctx->d_bstream.p, streams, (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(ctx->d_bpset.p, b.frame_set.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(ctx->d_brec.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemset(ctx->d_bstatus.p, 0, (size_t) nframes * sizeof(int)));
+  CU_TRY(b.d_bmax.reserve(nframes));
+  CU_TRY(b.d_bstream.reserve(nframes));
+  CU_TRY(b.d_bpset.reserve(nframes));
+  CU_TRY(b.d_bstatus.reserve(nframes));
+  CU_TRY(b.d_brec.reserve(nframes));
+  CU_TRY(cudaMemcpy(b.d_bmax.p, max_n, (size_t) nframes * sizeof(long long), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(b.d_bstream.p, streams, (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(b.d_bpset.p, b.frame_set.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(b.d_brec.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemset(b.d_bstatus.p, 0, (size_t) nframes * sizeof(int)));
   if (rings) {
     std::vector<BoundRing> ring(nframes);
     for (int f = 0; f < nframes; ++f)
       ring[f] = BoundRing{reinterpret_cast<const long long*>(rings[f].d_counts), (long long) rings[f].slot_stride, (int) rings[f].num_slots, 0};
-    CU_TRY(ctx->d_bring.reserve(nframes));
-    CU_TRY(ctx->d_bslot.reserve(nframes));
-    CU_TRY(ctx->d_brun.reserve(nframes));
-    CU_TRY(cudaMemcpy(ctx->d_bring.p, ring.data(), (size_t) nframes * sizeof(BoundRing), cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemcpy(ctx->d_brun.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemset(ctx->d_bslot.p, 0xff, (size_t) nframes * sizeof(int)));   // -1: no run yet
+    CU_TRY(b.d_bring.reserve(nframes));
+    CU_TRY(b.d_bslot.reserve(nframes));
+    CU_TRY(b.d_brun.reserve(nframes));
+    CU_TRY(cudaMemcpy(b.d_bring.p, ring.data(), (size_t) nframes * sizeof(BoundRing), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemcpy(b.d_brun.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemset(b.d_bslot.p, 0xff, (size_t) nframes * sizeof(int)));   // -1: no run yet
   }
   CU_TRY(cudaDeviceSynchronize());
   b.on = true;
@@ -1602,23 +1569,23 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   ctx->frame_set = b.frame_set;
   ctx->chunk_off = b.cap_chunk_off;
   ctx->pt_off = b.cap_pt_off;
-  const BoundActions A{b.d_actions, ctx->d_bact.p, ctx->d_bscratch.p, ctx->d_bdep.p, ctx->d_states_init.p, ctx->d_states.p};
-  const RecordFrame* recs = ctx->d_brec.p;   // the record table the unpack and the gather read
+  const BoundActions A{b.d_actions, b.d_bact.p, b.d_bscratch.p, b.d_bdep.p, ctx->d_states_init.p, ctx->d_states.p};
+  const RecordFrame* recs = b.d_brec.p;   // the record table the unpack and the gather read
   if (b.d_slots) {
-    const BoundRings G{b.d_slots, ctx->d_bslot.p, ctx->d_bring.p, ctx->d_brec.p, ctx->d_brun.p};
+    const BoundRings G{b.d_slots, b.d_bslot.p, b.d_bring.p, b.d_brec.p, b.d_brun.p};
     if (b.d_actions)
-      k_bound_table_rings_actions<<<1, BT_THREADS, 0, s>>>(nf, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
-                                                           ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p, A, G);
+      k_bound_table_rings_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                                           ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, A, G);
     else
-      k_bound_table_rings<<<1, BT_THREADS, 0, s>>>(nf, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
-                                                   ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p, G);
-    recs = ctx->d_brun.p;
+      k_bound_table_rings<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                                   ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, G);
+    recs = b.d_brun.p;
   } else if (b.d_actions) {
-    k_bound_table_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
-                                                   ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p, A);
+    k_bound_table_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                                   ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, A);
   } else {
-    k_bound_table<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, ctx->d_bmax.p, ctx->d_bstream.p, ctx->d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
-                                           ctx->d_stream.p, ctx->d_pset.p, ctx->d_bstatus.p);
+    k_bound_table<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                           ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p);
   }
   ++ctx->launches;
   if (b.unpack_gx > 0) {
@@ -1628,7 +1595,7 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   CU_TRY(cudaGetLastError());
   for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
     if (b.d_actions && b.reset_run[r]) {   // the RESET frames whose stream ran in an earlier run
-      k_bound_reset<<<1, BR_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], ctx->d_bact.p, ctx->d_bdep.p, ctx->d_bstream.p, ctx->d_states_init.p, ctx->d_states.p);
+      k_bound_reset<<<1, BR_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bact.p, b.d_bdep.p, b.d_bstream.p, ctx->d_states_init.p, ctx->d_states.p);
       ++ctx->launches;
       CU_TRY(cudaGetLastError());
     }
@@ -1636,7 +1603,7 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     if (rc) return rc;
     if (b.getters & PWPP_GETTER_STATE) {   // before a later run moves the run's streams
       const int len = b.runs[r + 1] - b.runs[r];
-      k_bound_states<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], ctx->d_bstream.p, ctx->d_states.p, ctx->d_bstates.p);
+      k_bound_states<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bstream.p, ctx->d_states.p, b.d_bstates.p);
       ++ctx->launches;
       CU_TRY(cudaGetLastError());
     }
@@ -1644,16 +1611,16 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   if (b.rec_parts) {   // the record results: both parts' lists are where the runs' k_emit left them
     const int first = b.rec_parts == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.rec_parts == 3 ? 2 : 1;
     k_gather_record_parts<<<dim3((unsigned) b.rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
-        recs, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, ctx->d_bpart_off.p, first, ctx->d_bground.p, ctx->d_bnonground.p,
-        ctx->d_rec_counts.p);
+        recs, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_bpart_off.p, first, b.d_bground.p, b.d_bnonground.p,
+        b.d_rec_counts.p);
     ++ctx->launches;
     CU_TRY(cudaGetLastError());
   }
   if (b.getters & (PWPP_GETTER_GROUND_XYZ | PWPP_GETTER_NONGROUND_XYZ)) {   // the xyz of both lists, from the unpacked points
     const int parts = b.getters & 3, first = parts == PWPP_GETTER_NONGROUND_XYZ ? 1 : 0, nparts = parts == 3 ? 2 : 1;
     k_gather_xyz_parts<<<dim3((unsigned) b.xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
-        ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, ctx->d_bxyz_off.p, first, ctx->d_bgxyz.p, ctx->d_bngxyz.p,
-        ctx->d_xyz_counts.p);
+        ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_bxyz_off.p, first, b.d_bgxyz.p, b.d_bngxyz.p,
+        b.d_xyz_counts.p);
     ++ctx->launches;
     CU_TRY(cudaGetLastError());
   }
@@ -1670,7 +1637,7 @@ int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int6
   if (d_indices) *d_indices = ctx->d_out_idx.p;
   if (d_offsets) *d_offsets = reinterpret_cast<const int64_t*>(ctx->d_pt_off.p);
   if (d_num_ground) *d_num_ground = ctx->d_counts.p;
-  if (d_status) *d_status = ctx->d_bstatus.p;
+  if (d_status) *d_status = ctx->bound.d_bstatus.p;
   return PWPP_OK;
 }
 
@@ -1678,7 +1645,7 @@ int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call_rings)");
   if (!ctx->bound.d_slots) return fail(PWPP_ERR_INVALID_ARG, "the bound call has no rings (pwpp_bind_call_rings)");
-  if (d_slots_read) *d_slots_read = ctx->d_bslot.p;
+  if (d_slots_read) *d_slots_read = ctx->bound.d_bslot.p;
   return PWPP_OK;
 }
 
@@ -1687,12 +1654,7 @@ int pwpp_unbind_call(pwpp_ctx* ctx) {
   if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound");
   int rc = bind_device(ctx);
   if (rc) return rc;
-  ctx->d_bmax.release(); ctx->d_bstream.release(); ctx->d_bpset.release(); ctx->d_bstatus.release(); ctx->d_brec.release();
-  ctx->d_bground.release(); ctx->d_bnonground.release(); ctx->d_bpart_off.release(); ctx->d_rec_counts.release();
-  ctx->d_bscratch.release(); ctx->d_bdep.release(); ctx->d_bact.release();
-  ctx->d_bring.release(); ctx->d_bslot.release(); ctx->d_brun.release();
-  ctx->d_bgxyz.release(); ctx->d_bngxyz.release(); ctx->d_bxyz_off.release(); ctx->d_xyz_counts.release(); ctx->d_bstates.release();
-  ctx->bound = pwpp_ctx::Bound();
+  ctx->bound = pwpp_ctx::Bound();   // releases the bound call's buffers
   return PWPP_OK;
 }
 
@@ -1708,12 +1670,12 @@ int pwpp_bind_record_results(pwpp_ctx* ctx, int parts) {
   std::vector<long long> off(nf + 1);   // the direct call's region layout with n = max_n
   rec_out_offsets(b.cap_pt_off.data(), b.recs.data(), nf, off.data());
   const size_t bytes = (size_t) std::max<long long>(off[nf], 16);
-  if (parts & PWPP_PART_GROUND) CU_TRY(ctx->d_bground.reserve(bytes));
-  if (parts & PWPP_PART_NONGROUND) CU_TRY(ctx->d_bnonground.reserve(bytes));
-  CU_TRY(ctx->d_bpart_off.reserve(nf + 1));
-  CU_TRY(ctx->d_rec_counts.reserve(2 * (size_t) nf));
-  CU_TRY(cudaMemcpy(ctx->d_bpart_off.p, off.data(), (size_t) (nf + 1) * sizeof(long long), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemset(ctx->d_rec_counts.p, 0, 2 * (size_t) nf * sizeof(int)));
+  if (parts & PWPP_PART_GROUND) CU_TRY(b.d_bground.reserve(bytes));
+  if (parts & PWPP_PART_NONGROUND) CU_TRY(b.d_bnonground.reserve(bytes));
+  CU_TRY(b.d_bpart_off.reserve(nf + 1));
+  CU_TRY(b.d_rec_counts.reserve(2 * (size_t) nf));
+  CU_TRY(cudaMemcpy(b.d_bpart_off.p, off.data(), (size_t) (nf + 1) * sizeof(long long), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemset(b.d_rec_counts.p, 0, 2 * (size_t) nf * sizeof(int)));
   CU_TRY(cudaDeviceSynchronize());
   b.rec_part_off = std::move(off);
   b.rec_gx = rec_parts_grid_x(b.cap_pt_off.data(), b.recs.data(), nf);
@@ -1727,10 +1689,10 @@ int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void**
   const pwpp_ctx::Bound& b = ctx->bound;
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (!b.rec_parts) return fail(PWPP_ERR_INVALID_ARG, "record results are not enabled for the bound call (pwpp_bind_record_results)");
-  if (d_ground) *d_ground = (b.rec_parts & PWPP_PART_GROUND) ? ctx->d_bground.p : nullptr;
-  if (d_nonground) *d_nonground = (b.rec_parts & PWPP_PART_NONGROUND) ? ctx->d_bnonground.p : nullptr;
+  if (d_ground) *d_ground = (b.rec_parts & PWPP_PART_GROUND) ? b.d_bground.p : nullptr;
+  if (d_nonground) *d_nonground = (b.rec_parts & PWPP_PART_NONGROUND) ? b.d_bnonground.p : nullptr;
   if (h_offsets) *h_offsets = reinterpret_cast<const int64_t*>(b.rec_part_off.data());
-  if (d_counts) *d_counts = ctx->d_rec_counts.p;
+  if (d_counts) *d_counts = b.d_rec_counts.p;
   return PWPP_OK;
 }
 
@@ -1744,17 +1706,17 @@ int pwpp_bind_getter_results(pwpp_ctx* ctx, int what) {
   if (rc) return rc;
   const int nf = b.nf;
   const size_t rows = (size_t) std::max<long long>(b.cap_pt_off[nf], 1);
-  if (what & PWPP_GETTER_GROUND_XYZ) CU_TRY(ctx->d_bgxyz.reserve(3 * rows));
-  if (what & PWPP_GETTER_NONGROUND_XYZ) CU_TRY(ctx->d_bngxyz.reserve(3 * rows));
+  if (what & PWPP_GETTER_GROUND_XYZ) CU_TRY(b.d_bgxyz.reserve(3 * rows));
+  if (what & PWPP_GETTER_NONGROUND_XYZ) CU_TRY(b.d_bngxyz.reserve(3 * rows));
   if (what & (PWPP_GETTER_GROUND_XYZ | PWPP_GETTER_NONGROUND_XYZ)) {
-    CU_TRY(ctx->d_bxyz_off.reserve(nf + 1));
-    CU_TRY(ctx->d_xyz_counts.reserve(2 * (size_t) nf));
-    CU_TRY(cudaMemcpy(ctx->d_bxyz_off.p, b.cap_pt_off.data(), (size_t) (nf + 1) * sizeof(long long), cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemset(ctx->d_xyz_counts.p, 0, 2 * (size_t) nf * sizeof(int)));
+    CU_TRY(b.d_bxyz_off.reserve(nf + 1));
+    CU_TRY(b.d_xyz_counts.reserve(2 * (size_t) nf));
+    CU_TRY(cudaMemcpy(b.d_bxyz_off.p, b.cap_pt_off.data(), (size_t) (nf + 1) * sizeof(long long), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemset(b.d_xyz_counts.p, 0, 2 * (size_t) nf * sizeof(int)));
   }
   if (what & PWPP_GETTER_STATE) {
-    CU_TRY(ctx->d_bstates.reserve(nf));
-    CU_TRY(cudaMemset(ctx->d_bstates.p, 0, (size_t) nf * sizeof(pwpp_state)));
+    CU_TRY(b.d_bstates.reserve(nf));
+    CU_TRY(cudaMemset(b.d_bstates.p, 0, (size_t) nf * sizeof(pwpp_state)));
   }
   CU_TRY(cudaDeviceSynchronize());
   b.xyz_gx = xyz_parts_grid_x(b.cap_pt_off.data(), nf);
@@ -1768,15 +1730,15 @@ int pwpp_bound_getter_results(pwpp_ctx* ctx, pwpp_bound_getters* out) {
   const pwpp_ctx::Bound& b = ctx->bound;
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   *out = pwpp_bound_getters{};
-  out->ground_xyz = (b.getters & PWPP_GETTER_GROUND_XYZ) ? ctx->d_bgxyz.p : nullptr;
-  out->nonground_xyz = (b.getters & PWPP_GETTER_NONGROUND_XYZ) ? ctx->d_bngxyz.p : nullptr;
+  out->ground_xyz = (b.getters & PWPP_GETTER_GROUND_XYZ) ? b.d_bgxyz.p : nullptr;
+  out->nonground_xyz = (b.getters & PWPP_GETTER_NONGROUND_XYZ) ? b.d_bngxyz.p : nullptr;
   out->h_row_off = reinterpret_cast<const int64_t*>(b.cap_pt_off.data());
-  out->xyz_counts = (b.getters & 3) ? ctx->d_xyz_counts.p : nullptr;
+  out->xyz_counts = (b.getters & 3) ? b.d_xyz_counts.p : nullptr;
   out->centers = ctx->d_centers.p;
   out->normals = ctx->d_normals.p;
   out->num_patches = ctx->d_counts.p + b.nf;   // row 1 of the count rows of the bound call
   out->patch_row_stride = ctx->gs.nbs;
-  out->states = (b.getters & PWPP_GETTER_STATE) ? ctx->d_bstates.p : nullptr;
+  out->states = (b.getters & PWPP_GETTER_STATE) ? b.d_bstates.p : nullptr;
   return PWPP_OK;
 }
 
@@ -1850,10 +1812,8 @@ static int copy_records(pwpp_ctx* ctx, int f, void* dst, bool ground) {
   rc = fetch_records(ctx);
   if (rc) return rc;
   const long long step = ctx->last_recs[f].step;
-  const int ng = ctx->h_counts.p[f];
-  const int nn = frame_n(ctx, f) - ng - count_of(ctx, 2, f);
-  const long long cnt = ground ? ng : nn;
-  if (cnt > 0) std::memcpy(dst, ctx->h_rec_out.p + ctx->rec_off[f] + (ground ? 0 : (long long) ng * step), (size_t) (cnt * step));
+  const FrameList L = frame_list(ctx, f, ground);
+  if (L.count > 0) std::memcpy(dst, ctx->h_rec_out.p + ctx->rec_off[f] + L.start * step, (size_t) (L.count * step));
   return PWPP_OK;
 }
 int pwpp_copy_ground_records(pwpp_ctx* ctx, int f, void* dst) { return copy_records(ctx, f, dst, true); }
@@ -1881,39 +1841,30 @@ int64_t pwpp_num_ground(pwpp_ctx* ctx, int f) {
 }
 int64_t pwpp_num_nonground(pwpp_ctx* ctx, int f) {
   if (check_frame(ctx, f) || fetch_counts(ctx)) return -1;
-  return (int64_t) frame_n(ctx, f) - ctx->h_counts.p[f] - count_of(ctx, 2, f);
+  return frame_list(ctx, f, false).count;
 }
-int pwpp_copy_ground_indices(pwpp_ctx* ctx, int f, int32_t* dst) {
+static int copy_indices(pwpp_ctx* ctx, int f, int32_t* dst, bool ground) {
   int rc = check_frame(ctx, f);
   if (rc) return rc;
   rc = fetch_indices(ctx);
   if (rc) return rc;
-  const int ng = ctx->h_counts.p[f];
-  if (ng > 0) std::memcpy(dst, ctx->h_out_idx.p + ctx->pt_off[f], (size_t) ng * sizeof(int32_t));
+  const FrameList L = frame_list(ctx, f, ground);
+  if (L.count > 0) std::memcpy(dst, ctx->h_out_idx.p + ctx->pt_off[f] + L.start, (size_t) L.count * sizeof(int32_t));
   return PWPP_OK;
 }
-int pwpp_copy_nonground_indices(pwpp_ctx* ctx, int f, int32_t* dst) {
-  int rc = check_frame(ctx, f);
-  if (rc) return rc;
-  rc = fetch_indices(ctx);
-  if (rc) return rc;
-  const int ng = ctx->h_counts.p[f];
-  const int nn = frame_n(ctx, f) - ng - count_of(ctx, 2, f);
-  if (nn > 0) std::memcpy(dst, ctx->h_out_idx.p + ctx->pt_off[f] + ng, (size_t) nn * sizeof(int32_t));
-  return PWPP_OK;
-}
+int pwpp_copy_ground_indices(pwpp_ctx* ctx, int f, int32_t* dst) { return copy_indices(ctx, f, dst, true); }
+int pwpp_copy_nonground_indices(pwpp_ctx* ctx, int f, int32_t* dst) { return copy_indices(ctx, f, dst, false); }
 
 static int copy_xyz(pwpp_ctx* ctx, int f, float* dst, bool ground) {
   int rc = check_frame(ctx, f);
   if (rc) return rc;
   rc = fetch_counts(ctx);
   if (rc) return rc;
-  const int ng = ctx->h_counts.p[f];
-  const int nn = frame_n(ctx, f) - ng - count_of(ctx, 2, f);
-  const int cnt = ground ? ng : nn;
+  const FrameList L = frame_list(ctx, f, ground);
+  const int cnt = L.count;
   if (cnt <= 0) return PWPP_OK;
   CU_TRY(ctx->d_xyz.reserve((size_t) cnt * 3));
-  const int* idx = ctx->d_out_idx.p + ctx->pt_off[f] + (ground ? 0 : ng);
+  const int* idx = ctx->d_out_idx.p + ctx->pt_off[f] + L.start;
   k_gather_xyz<<<(cnt + 255) / 256, 256, 0, ctx->last_stream>>>(ctx->last_pts + ctx->pt_off[f], idx, cnt, ctx->d_xyz.p);
   CU_TRY(cudaGetLastError());
   CU_TRY(cudaMemcpyAsync(dst, ctx->d_xyz.p, (size_t) cnt * 3 * sizeof(float), cudaMemcpyDeviceToHost, ctx->last_stream));
