@@ -416,6 +416,63 @@ int pwpp_bind_call_rings(pwpp_ctx* ctx, int nframes, const int32_t* streams, con
                          const int64_t* max_n, const pwpp_point_layout* layouts, const int32_t* d_slots /* device [nframes] */,
                          const int32_t* d_actions /* NULL: all RUN */);
 int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read);
+
+/* Packed batches of a bound call: all frames back to back in one buffer, frame f at records [d_offsets[f], d_offsets[f + 1]),
+ * the layout of torch.nested's jagged tensors, of PyG's ptr and of any stream compaction over a whole batch. The offsets live
+ * on the device and may change at every tick, so where every frame starts is decided on the GPU at every run or replay, with
+ * no scatter into fixed per-frame buffers.
+ *
+ * pwpp_bind_call_packed: pwpp_bind_call_actions with the frames in one packed buffer. base holds capacity records of *layout
+ * (one point_step for the whole buffer, any alignment). d_offsets is a device int64 array of nframes + 1 entries that the GPU
+ * reads at every run or replay; max_n[f] keeps its meaning (it bounds frame f's count and sizes the grids). d_actions as for
+ * pwpp_bind_call_actions (NULL: all RUN).
+ *   - Reading the offsets. On every run or replay, frame f reads lo = d_offsets[f] and hi = d_offsets[f + 1] in the run's first
+ *     kernel. If lo < 0, hi < lo or hi > capacity, d_status[f] = PWPP_OFFSETS_OUT_OF_RANGE: the frame runs as an empty frame and
+ *     its stream advances as after an empty call. Otherwise a count hi - lo above max_n[f] gives PWPP_COUNT_OUT_OF_RANGE and an
+ *     empty frame. Otherwise the frame is the hi - lo records at base + lo * point_step. Each frame is judged by its own two
+ *     entries only.
+ *   - Precedence. A frame whose action skips it reads neither offset (status PWPP_FRAME_SKIPPED or PWPP_ACTION_INVALID). A
+ *     RESET still applies when the frame's offsets turn out invalid.
+ *   - What is read. No byte outside [base, base + capacity * point_step) is read, whatever d_offsets holds.
+ *   - Results. Everything else is as for pwpp_bind_call_actions: the stream table and run split, the record results, the getter
+ *     results, the freeze and pwpp_unbind_call. The index lists stay frame-relative (index k of frame f is record lo + k).
+ *   - The caller's obligation. Between a run's first kernel and the end of its last kernel, the caller must not write the offsets
+ *     or the records of the frames the run reads.
+ *   - Bind-time checks, before anything is allocated, each message naming the frame or the field (PWPP_ERR_INVALID_ARG or
+ *     PWPP_ERR_UNSUPPORTED): every check of pwpp_bind_call with frames[f] = base, layouts[f] = *layout and n = max_n[f]; NULL
+ *     layout or d_offsets; NULL base with capacity > 0; capacity < 0; capacity * point_step or its end address overflowing.
+ *   - Work buffers are reserved for sum(max_n) points, as for pwpp_bind_call. Accepted frames may overlap in the buffer (a
+ *     decreasing offset makes its frame invalid, and a skipped frame validates neither of its entries, so the frames around it
+ *     can share records), so the accepted counts of one run are bounded by sum(max_n), not by capacity.
+ *   - pwpp_launch_count rises exactly as for the same call bound with pwpp_bind_call_actions: there is no extra launch.
+ *   - Identity. With frames[f] = base + d_offsets[f] * point_step and d_counts[f] = d_offsets[f + 1] - d_offsets[f] (valid
+ *     offsets), pwpp_bind_call_actions gives the same results bit for bit: indices, offsets, status, patches, states, record and
+ *     getter results.
+ *   - Memory: 48 + 48 bytes per frame on the device, next to the bound call's other tables.
+ *
+ * Packed xyz results of a bound call, for a consumer that takes one packed tensor with offsets rather than the capacity layout of
+ * pwpp_bound_getters.
+ *
+ * pwpp_bind_packed_xyz: enables them for any bound call (plain, with actions, rings or packed). parts is PWPP_PART_GROUND,
+ * PWPP_PART_NONGROUND or both (3). Host work that synchronizes, like pwpp_bind_getter_results, so it is not capturable; graphs
+ * captured before it do not write these results. PWPP_ERR_INVALID_ARG when no call is bound, for parts outside {1, 2, 3}, and
+ * when packed xyz is already enabled (one setting per bind: pwpp_unbind_call releases the buffers).
+ *   - Layout. Per enabled part, a float32 buffer of rows of 3 and a device int64[nframes + 1] offsets array, the exclusive scan of
+ *     that part's per-frame counts in the run. After every run or replay frame f's ground rows are ground[g_off[f] : g_off[f+1]]
+ *     and its non-ground rows nonground[ng_off[f] : ng_off[f + 1]]. Row k of a frame is row k of pwpp_copy_ground_xyz /
+ *     pwpp_copy_nonground_xyz of that frame, bit for bit, in the order the call was bound with. Skipped frames and frames with an
+ *     invalid count, slot or offsets have count 0. Rows past off[nframes] are never written.
+ *   - Independent of the getter results: both can be enabled, and each writes its own buffers.
+ *   - pwpp_launch_count rises, per pwpp_run_bound_call, by two launches after the last run's output kernel (the offset scan and
+ *     the gather), also when every max_n is 0.
+ *   - Memory: 12 sum(max_n) bytes per enabled part plus 16 (nframes + 1) bytes of offsets.
+ *
+ * pwpp_bound_packed_xyz: host-only. The fixed device pointers of both buffers and both offsets arrays (NULL for a part that is
+ * not enabled). PWPP_ERR_INVALID_ARG when no call is bound or packed xyz is not enabled. */
+#define PWPP_OFFSETS_OUT_OF_RANGE 5   /* d_status[f]: d_offsets[f], d_offsets[f + 1] not 0 <= lo <= hi <= capacity; empty frame */
+int pwpp_bind_call_packed(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* base, const pwpp_point_layout* layout,
+                          int64_t capacity /* records at base */, const int64_t* max_n, const int64_t* d_offsets /* device [nframes + 1] */,
+                          const int32_t* d_actions /* NULL: all RUN */);
 int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream);
 int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int64_t** d_offsets, const int32_t** d_num_ground,
                             const int32_t** d_status);
@@ -424,6 +481,9 @@ int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int6
 int pwpp_bind_record_results(pwpp_ctx* ctx, int parts /* PWPP_PART_* bits: 1, 2 or 3 */);
 int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void** d_nonground, const int64_t** h_offsets,
                               const int32_t** d_counts);
+int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts /* PWPP_PART_* bits: 1, 2 or 3 */);
+int pwpp_bound_packed_xyz(pwpp_ctx* ctx, const float** d_ground, const float** d_nonground, const int64_t** d_ground_off,
+                          const int64_t** d_nonground_off);
 
 /* Getter results of the bound call: what the reference's other getters return (getGround / getNonground, getCenters /
  * getNormals, getHeight and the adaptive thresholds, H:154-163), at fixed device addresses, for a graph whose next stage takes

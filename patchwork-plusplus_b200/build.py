@@ -110,6 +110,12 @@ def build_examples(force=False):
     if force or _newer(out9, [src9] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out9, src9])
+    # the kernels of a bound call's packed xyz results, the same way (GPU cases of tests/test_bound_packed_xyz_backends.py)
+    src10 = os.path.join(REPO, "tests", "gpu_bound_packed_probe.cu")
+    out10 = os.path.join(LIB, "libpwpp_bound_packed_probe.so")
+    if force or _newer(out10, [src10] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out10, src10])
     return out
 
 

@@ -266,13 +266,18 @@ struct pwpp_ctx {
     const int* d_slots = nullptr;           // the caller's device slots (pwpp_bind_call_rings), NULL: no rings
     DevBuf<BoundRing, false> d_bring;       // [F] with rings: every frame's ring
     DevBuf<int, false> d_bslot;             // [F] the run's copy of the slots
-    DevBuf<RecordFrame, false> d_brun;      // [F] the run's record table (d_brec with every frame's slot applied)
+    DevBuf<RecordFrame, false> d_brun;      // [F] the run's record table (d_brec with every frame's slot or offset applied)
+    const long long* d_offsets = nullptr;   // the caller's device offsets (pwpp_bind_call_packed), NULL: not packed
+    long long capacity = 0;                 // records at the packed buffer's base
     int getters = 0;                        // getter results (pwpp_bind_getter_results): PWPP_GETTER_* bits, 0 = off
     long long xyz_gx = 0;                   // grid.x of k_gather_xyz_parts, from the capacities
     DevBuf<float, false> d_bgxyz, d_bngxyz;  // getter results: [sum(max_n)][3] ground / non-ground xyz, frame f from row cap_pt_off[f]
     DevBuf<long long, false> d_bxyz_off;    // [F+1] cap_pt_off
     DevBuf<int, false> d_xyz_counts;        // [F][2]: ground, non-ground xyz rows of every frame of the last run
     DevBuf<pwpp_state, false> d_bstates;    // [F] the state of every frame's stream right after the frame
+    int packed_xyz = 0;                     // packed xyz results (pwpp_bind_packed_xyz): PWPP_PART_* bits, 0 = off
+    DevBuf<float, false> d_pgxyz, d_pngxyz;  // [sum(max_n)][3] packed ground / non-ground xyz
+    DevBuf<long long, false> d_pg_off, d_png_off;   // [F+1] their row offsets, scanned on the device at every run
   } bound;
   int scratch_slots = 0;                  // state / history slots after the streams' (pwpp_bind_call_actions), kept after unbind
 
@@ -990,6 +995,9 @@ static int create_impl(const pwpp_params* sets, int num_sets, const int32_t* str
     CU_TRY_CTX(cudaMemcpy(ctx->d_states_init.p, v.data(), v.size() * sizeof(StreamState), cudaMemcpyHostToDevice));
   }
   CU_TRY_CTX(ctx->d_hist.reserve((size_t) num_streams * 2 * 4 * ctx->hist_stride));
+  // history samples past a stream's counts are never read by the kernels, but pwpp_export_state copies whole rows: zeroed, a
+  // blob holds no bytes of whatever the allocation held before
+  CU_TRY_CTX(cudaMemset(ctx->d_hist.p, 0, (size_t) num_streams * 2 * 4 * ctx->hist_stride * sizeof(double)));
   CU_TRY_CTX(ctx->d_counts.reserve((size_t) 3 * num_streams));
   CU_TRY_CTX(ctx->d_wq_ctr.reserve(2 * NUM_CLASSES + ORD_NUM_HEADS));
   {
@@ -1418,22 +1426,37 @@ static int check_rings(int nframes, const pwpp_scan_ring* rings, const int64_t* 
   return PWPP_OK;
 }
 
-// The bind of pwpp_bind_call, pwpp_bind_call_actions and pwpp_bind_call_rings. rings is NULL for the first two; with rings,
-// frames[f] is rings[f].base and d_counts is unused.
+// The checks of a packed bind beyond those of pwpp_bind_call (frames[f] = base): the buffer's extent. They run before the records
+// checks, so that a NULL base is named as such.
+static int check_packed(const void* base, int64_t capacity, const pwpp_point_layout& layout) {
+  if (capacity < 0) return fail(PWPP_ERR_INVALID_ARG, "capacity " + std::to_string(capacity) + " < 0");
+  if (!base && capacity > 0) return fail(PWPP_ERR_INVALID_ARG, "base is NULL with capacity " + std::to_string(capacity) + " > 0");
+  // the kernels form base + lo * point_step in 64 bits: the extent and its end address must not overflow
+  const __int128 extent = (__int128) capacity * layout.point_step;
+  if (extent > (__int128) INT64_MAX || (__int128) (uintptr_t) base + extent > (__int128) UINTPTR_MAX)
+    return fail(PWPP_ERR_INVALID_ARG, "capacity * point_step (" + std::to_string(capacity) + " * " + std::to_string(layout.point_step) + ") overflows");
+  return PWPP_OK;
+}
+
+// The bind of pwpp_bind_call, pwpp_bind_call_actions, pwpp_bind_call_rings and pwpp_bind_call_packed. rings is NULL except for
+// the ring bind, where frames[f] is rings[f].base and d_counts is unused; d_offsets is NULL except for the packed bind, where
+// frames[f] is its base, layouts[f] its layout and d_counts is unused.
 // With actions: frame f of run r gets scratch slot num_streams + (f - runs[r]) (distinct inside a run), and dep[f] says whether
 // its stream has a frame in an earlier run (then a RESET of f waits for that run: k_bound_reset before f's run).
 static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* const* frames, const int64_t* max_n,
                           const pwpp_point_layout* layouts, const int64_t* d_counts, const int32_t* d_actions, const pwpp_scan_ring* rings,
-                          const int32_t* d_slots) {
+                          const int32_t* d_slots, const int64_t* d_offsets = nullptr, int64_t capacity = 0) {
   int rc = check_records_call(ctx, nframes, streams, frames, max_n, layouts);
   if (rc) return rc;
   if (ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "a call is already bound (pwpp_unbind_call releases it)");
-  if (!rings && !d_counts) return fail(PWPP_ERR_INVALID_ARG, "d_counts is NULL");
+  if (!rings && !d_offsets && !d_counts) return fail(PWPP_ERR_INVALID_ARG, "d_counts is NULL");
   if (rings && (rc = check_rings(nframes, rings, max_n, layouts))) return rc;
   pwpp_ctx::Bound b;
   b.nf = nframes;
   b.d_counts = reinterpret_cast<const long long*>(d_counts);
   b.d_slots = d_slots;
+  b.d_offsets = reinterpret_cast<const long long*>(d_offsets);
+  b.capacity = capacity;
   b.cap_pt_off.assign(nframes + 1, 0);
   b.cap_chunk_off.assign(nframes + 1, 0);
   long long chunks = 0;
@@ -1531,6 +1554,10 @@ static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
     CU_TRY(cudaMemcpy(b.d_brun.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
     CU_TRY(cudaMemset(b.d_bslot.p, 0xff, (size_t) nframes * sizeof(int)));   // -1: no run yet
   }
+  if (d_offsets) {
+    CU_TRY(b.d_brun.reserve(nframes));
+    CU_TRY(cudaMemcpy(b.d_brun.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
+  }
   CU_TRY(cudaDeviceSynchronize());
   b.on = true;
   ctx->bound = std::move(b);
@@ -1550,6 +1577,18 @@ int pwpp_bind_call_rings(pwpp_ctx* ctx, int nframes, const int32_t* streams, con
   std::vector<const void*> frames(std::max(nframes, 1), nullptr);
   for (int f = 0; f < nframes; ++f) frames[f] = rings[f].base;
   return bind_call_impl(ctx, nframes, streams, frames.data(), max_n, layouts, nullptr, d_actions, rings, d_slots);
+}
+
+int pwpp_bind_call_packed(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* base, const pwpp_point_layout* layout,
+                          int64_t capacity, const int64_t* max_n, const int64_t* d_offsets, const int32_t* d_actions) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!layout) return fail(PWPP_ERR_INVALID_ARG, "layout is NULL");
+  if (!d_offsets) return fail(PWPP_ERR_INVALID_ARG, "d_offsets is NULL");
+  const int rc = check_packed(base, capacity, *layout);
+  if (rc) return rc;
+  std::vector<const void*> frames(std::max(nframes, 1), base);
+  std::vector<pwpp_point_layout> layouts(std::max(nframes, 1), *layout);
+  return bind_call_impl(ctx, nframes, streams, frames.data(), max_n, layouts.data(), nullptr, d_actions, nullptr, nullptr, d_offsets, capacity);
 }
 
 // One table launch, one unpack launch (capacities with points), then every run through launch_range_impl with grids sized for
@@ -1579,6 +1618,15 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     else
       k_bound_table_rings<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
                                                    ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, G);
+    recs = b.d_brun.p;
+  } else if (b.d_offsets) {
+    const BoundPacked P{b.d_offsets, b.capacity, b.d_brec.p, b.d_brun.p};
+    if (b.d_actions)
+      k_bound_table_packed_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                                            ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, A, P);
+    else
+      k_bound_table_packed<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
+                                                    ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, P);
     recs = b.d_brun.p;
   } else if (b.d_actions) {
     k_bound_table_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
@@ -1622,6 +1670,14 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
         ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_bxyz_off.p, first, b.d_bgxyz.p, b.d_bngxyz.p,
         b.d_xyz_counts.p);
     ++ctx->launches;
+    CU_TRY(cudaGetLastError());
+  }
+  if (b.packed_xyz) {   // the offsets of both parts from the final counts, then the rows
+    k_bound_xyz_offsets<<<1, BT_THREADS, 0, s>>>(nf, ctx->d_pt_off.p, ctx->d_counts.p, b.d_pg_off.p, b.d_png_off.p);
+    const int first = b.packed_xyz == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.packed_xyz == 3 ? 2 : 1;
+    k_gather_xyz_packed<<<dim3((unsigned) b.xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
+        ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_pg_off.p, b.d_png_off.p, first, b.d_pgxyz.p, b.d_pngxyz.p);
+    ctx->launches += 2;
     CU_TRY(cudaGetLastError());
   }
   make_bound_last(ctx, s);
@@ -1721,6 +1777,42 @@ int pwpp_bind_getter_results(pwpp_ctx* ctx, int what) {
   CU_TRY(cudaDeviceSynchronize());
   b.xyz_gx = xyz_parts_grid_x(b.cap_pt_off.data(), nf);
   b.getters = what;
+  return PWPP_OK;
+}
+
+int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
+  if (b.packed_xyz) return fail(PWPP_ERR_INVALID_ARG, "packed xyz is already enabled for the bound call");
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const int nf = b.nf;
+  const size_t rows = (size_t) std::max<long long>(b.cap_pt_off[nf], 1);
+  if (parts & PWPP_PART_GROUND) CU_TRY(b.d_pgxyz.reserve(3 * rows));
+  if (parts & PWPP_PART_NONGROUND) CU_TRY(b.d_pngxyz.reserve(3 * rows));
+  CU_TRY(b.d_pg_off.reserve(nf + 1));
+  CU_TRY(b.d_png_off.reserve(nf + 1));
+  CU_TRY(cudaMemset(b.d_pg_off.p, 0, (size_t) (nf + 1) * sizeof(long long)));
+  CU_TRY(cudaMemset(b.d_png_off.p, 0, (size_t) (nf + 1) * sizeof(long long)));
+  CU_TRY(cudaDeviceSynchronize());
+  b.xyz_gx = xyz_parts_grid_x(b.cap_pt_off.data(), nf);
+  b.packed_xyz = parts;
+  return PWPP_OK;
+}
+
+int pwpp_bound_packed_xyz(pwpp_ctx* ctx, const float** d_ground, const float** d_nonground, const int64_t** d_ground_off,
+                          const int64_t** d_nonground_off) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  const pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (!b.packed_xyz) return fail(PWPP_ERR_INVALID_ARG, "packed xyz is not enabled for the bound call (pwpp_bind_packed_xyz)");
+  const bool g = b.packed_xyz & PWPP_PART_GROUND, n = b.packed_xyz & PWPP_PART_NONGROUND;
+  if (d_ground) *d_ground = g ? b.d_pgxyz.p : nullptr;
+  if (d_nonground) *d_nonground = n ? b.d_pngxyz.p : nullptr;
+  if (d_ground_off) *d_ground_off = g ? reinterpret_cast<const int64_t*>(b.d_pg_off.p) : nullptr;
+  if (d_nonground_off) *d_nonground_off = n ? reinterpret_cast<const int64_t*>(b.d_png_off.p) : nullptr;
   return PWPP_OK;
 }
 

@@ -155,7 +155,43 @@ inline RecordFrame record_frame(const pwpp_point_layout& L, const void* src) {
 // from its ring's counts[s] and writes the run's record table entry brun[f] = the bound entry brec[f] with src = base +
 // s * stride. A slot outside [0, num_slots) makes an empty frame with status PWPP_SLOT_OUT_OF_RANGE; skipped frames and those
 // keep src = base with n = 0, so nothing is read. The unpack and the record gather of the run read brun.
+//
+// With a packed buffer (pwpp_bind_call_packed), k_bound_table_packed / k_bound_table_packed_actions pick every frame's records
+// from the caller's device offsets: a frame that runs reads lo = offsets[f] and hi = offsets[f + 1]; offsets outside
+// 0 <= lo <= hi <= capacity make an empty frame with status PWPP_OFFSETS_OUT_OF_RANGE, a count hi - lo above max_n[f] one with
+// PWPP_COUNT_OUT_OF_RANGE, and an accepted frame's entry brun[f] is brec[f] with src = base + lo * step. Every other frame keeps
+// src = base with n = 0. A skipped frame reads neither offset.
 constexpr int BT_THREADS = 1024;
+
+// The CTA-wide scan of the one-CTA table kernels (bound_table_body, k_bound_xyz_offsets): each of the BT_THREADS threads (lane,
+// warp) brings the sums own_a, own_b of its slice of frames and gets back in a, b their exclusive prefix sums, the start of its
+// slice: a warp-shuffle scan, then one of the warp totals in s_a, s_b (BT_THREADS / 32 entries each).
+template <typename A, typename B>
+__device__ __forceinline__ void bt_scan_slices(int lane, int warp, A own_a, B own_b, A& a, B& b, A* s_a, B* s_b) {
+  A pa = own_a;   // inclusive scan over the warp's slices
+  B pb = own_b;
+  for (int d = 1; d < 32; d <<= 1) {
+    const A p = __shfl_up_sync(0xffffffffu, pa, d);
+    const B q = __shfl_up_sync(0xffffffffu, pb, d);
+    if (lane >= d) { pa += p; pb += q; }
+  }
+  if (lane == 31) { s_a[warp] = pa; s_b[warp] = pb; }
+  __syncthreads();
+  if (warp == 0) {   // inclusive scan of the warp totals
+    A wa = s_a[lane];
+    B wb = s_b[lane];
+    for (int d = 1; d < 32; d <<= 1) {
+      const A p = __shfl_up_sync(0xffffffffu, wa, d);
+      const B q = __shfl_up_sync(0xffffffffu, wb, d);
+      if (lane >= d) { wa += p; wb += q; }
+    }
+    s_a[lane] = wa;
+    s_b[lane] = wb;
+  }
+  __syncthreads();
+  a = (warp > 0 ? s_a[warp - 1] : 0) + pa - own_a;
+  b = (warp > 0 ? s_b[warp - 1] : 0) + pb - own_b;
+}
 
 struct BoundActions {
   const int* actions;            // the caller's device actions [nf]
@@ -206,12 +242,28 @@ __device__ __forceinline__ long long bt_count(const long long* __restrict__ coun
   return bt_slot_ok(s, R) ? R.counts[s] : -1;
 }
 
-template <bool Actions, bool Rings = false>
+// the packed buffer of a bound call (pwpp_bind_call_packed)
+struct BoundPacked {
+  const long long* offsets;      // the caller's device offsets [nf + 1]
+  long long capacity;            // records at the bound base
+  const RecordFrame* brec;       // the bound record table (src: base)
+  RecordFrame* brun;             // the run's record table
+};
+
+__device__ __forceinline__ bool bt_offsets_ok(long long lo, long long hi, long long capacity) { return lo >= 0 && hi >= lo && hi <= capacity; }
+
+// frame f's count from its two offsets, -1 (an empty frame) for offsets out of range
+__device__ __forceinline__ long long bt_packed_count(const BoundPacked& P, int f) {
+  const long long lo = P.offsets[f], hi = P.offsets[f + 1];
+  return bt_offsets_ok(lo, hi, P.capacity) ? hi - lo : -1;
+}
+
+template <bool Actions, bool Rings = false, bool Packed = false>
 __device__ __forceinline__ void bound_table_body(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
                                                  const int* __restrict__ b_stream, const int* __restrict__ b_pset, long long* __restrict__ pt_off,
                                                  int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
                                                  int* __restrict__ status, const BoundActions& A, long long* s_pts, int* s_chk,
-                                                 const BoundRings& G = BoundRings{}) {
+                                                 const BoundRings& G = BoundRings{}, const BoundPacked& P = BoundPacked{}) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int per = (nf + BT_THREADS - 1) / BT_THREADS;
   const int f0 = tid * per < nf ? tid * per : nf;
@@ -221,7 +273,7 @@ __device__ __forceinline__ void bound_table_body(int nf, const long long* __rest
   for (int f = f0; f < f1; ++f) {
     long long n = 0;
     if (bt_runs(bt_action<Actions>(A, f))) {
-      const long long c = bt_count<Rings>(counts, G, f);
+      const long long c = Packed ? bt_packed_count(P, f) : bt_count<Rings>(counts, G, f);
       n = (c >= 0 && c <= max_n[f]) ? c : 0;
     } else if (Rings) {
       G.slot[f] = -1;
@@ -229,29 +281,9 @@ __device__ __forceinline__ void bound_table_body(int nf, const long long* __rest
     own_pts += n;
     own_chk += (int) ((n + CHUNK_PTS - 1) / CHUNK_PTS);
   }
-  long long pts = own_pts;   // inclusive scan over the warp's slices
-  int chk = own_chk;
-  for (int d = 1; d < 32; d <<= 1) {
-    const long long p = __shfl_up_sync(0xffffffffu, pts, d);
-    const int q = __shfl_up_sync(0xffffffffu, chk, d);
-    if (lane >= d) { pts += p; chk += q; }
-  }
-  if (lane == 31) { s_pts[warp] = pts; s_chk[warp] = chk; }
-  __syncthreads();
-  if (warp == 0) {   // inclusive scan of the warp totals
-    long long wp = s_pts[lane];
-    int wc = s_chk[lane];
-    for (int d = 1; d < 32; d <<= 1) {
-      const long long p = __shfl_up_sync(0xffffffffu, wp, d);
-      const int q = __shfl_up_sync(0xffffffffu, wc, d);
-      if (lane >= d) { wp += p; wc += q; }
-    }
-    s_pts[lane] = wp;
-    s_chk[lane] = wc;
-  }
-  __syncthreads();
-  long long p = (warp > 0 ? s_pts[warp - 1] : 0) + pts - own_pts;   // start of the slice
-  int q = (warp > 0 ? s_chk[warp - 1] : 0) + chk - own_chk;
+  long long p;   // the start of the slice
+  int q;
+  bt_scan_slices(lane, warp, own_pts, own_chk, p, q, s_pts, s_chk);
   for (int f = f0; f < f1; ++f) {
     if (Actions) {
       const int a = A.act[f];   // this thread's own copy from the first pass
@@ -262,6 +294,7 @@ __device__ __forceinline__ void bound_table_body(int nf, const long long* __rest
         stream[f] = A.scratch[f];
         pset[f] = b_pset[f];
         if (Rings) G.brun[f] = G.brec[f];
+        if (Packed) P.brun[f] = P.brec[f];
         continue;
       }
       if (a == PWPP_FRAME_RESET && !A.dep[f]) A.states[b_stream[f]] = A.init[b_stream[f]];
@@ -280,6 +313,17 @@ __device__ __forceinline__ void bound_table_body(int nf, const long long* __rest
         bad = PWPP_SLOT_OUT_OF_RANGE;
       }
       G.brun[f] = r;
+    } else if (Packed) {
+      const long long lo = P.offsets[f], hi = P.offsets[f + 1];
+      if (bt_offsets_ok(lo, hi, P.capacity)) {
+        c = hi - lo;
+      } else {
+        c = -1;
+        bad = PWPP_OFFSETS_OUT_OF_RANGE;
+      }
+      RecordFrame r = P.brec[f];
+      if (c >= 0 && c <= max_n[f]) r.src += lo * r.step;
+      P.brun[f] = r;
     } else {
       c = counts[f];
     }
@@ -330,6 +374,25 @@ __global__ void __launch_bounds__(BT_THREADS) k_bound_table_rings_actions(int nf
   __shared__ long long s_pts[BT_THREADS / 32];
   __shared__ int s_chk[BT_THREADS / 32];
   bound_table_body<true, true>(nf, nullptr, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk, G);
+}
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table_packed(int nf, const long long* __restrict__ max_n, const int* __restrict__ b_stream,
+                                                                   const int* __restrict__ b_pset, long long* __restrict__ pt_off,
+                                                                   int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
+                                                                   int* __restrict__ status, const BoundPacked P) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<false, false, true>(nf, nullptr, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, BoundActions{}, s_pts, s_chk,
+                                       BoundRings{}, P);
+}
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table_packed_actions(int nf, const long long* __restrict__ max_n, const int* __restrict__ b_stream,
+                                                                           const int* __restrict__ b_pset, long long* __restrict__ pt_off,
+                                                                           int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
+                                                                           int* __restrict__ status, const BoundActions A, const BoundPacked P) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<true, false, true>(nf, nullptr, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk, BoundRings{}, P);
 }
 
 // k_bound_reset: one CTA before run [f0, f1) of a bound call with actions, launched only for runs that hold a frame whose stream

@@ -78,6 +78,9 @@ def load_library():
     lib.pwpp_bind_call_actions.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]; lib.pwpp_bind_call_actions.restype = i32
     lib.pwpp_bind_call_rings.argtypes = [vp, i32, vp, C.POINTER(PwppScanRing), vp, vp, vp, vp]; lib.pwpp_bind_call_rings.restype = i32
     lib.pwpp_bound_call_slots.argtypes = [vp, C.POINTER(vp)]; lib.pwpp_bound_call_slots.restype = i32
+    lib.pwpp_bind_call_packed.argtypes = [vp, i32, vp, vp, C.POINTER(PwppPointLayout), i64, vp, vp, vp]; lib.pwpp_bind_call_packed.restype = i32
+    lib.pwpp_bind_packed_xyz.argtypes = [vp, i32]; lib.pwpp_bind_packed_xyz.restype = i32
+    lib.pwpp_bound_packed_xyz.argtypes = [vp] + [C.POINTER(vp)] * 4; lib.pwpp_bound_packed_xyz.restype = i32
     lib.pwpp_run_bound_call.argtypes = [vp, vp]; lib.pwpp_run_bound_call.restype = i32
     lib.pwpp_bound_call_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_bound_call_results.restype = i32
     lib.pwpp_unbind_call.argtypes = [vp]; lib.pwpp_unbind_call.restype = i32
@@ -366,6 +369,67 @@ class Engine:
         self._bound = ([r[0] for r in rings], None, ids.tolist(), sum(int(k) for k in max_n))
         self._bound_actions = actions
         self._bound_rings = (list(rings), slots)
+
+    def bind_call_packed(self, points, offsets, max_n, layout=None, streams=None, actions=None):
+        """Binds a call over one packed batch (pwpp_bind_call_packed): at every run or replay frame f is records
+        [offsets[f], offsets[f + 1]) of `points`, read by the GPU. `points` is a contiguous CUDA tensor; a float32 (N, 4) or (N, 3)
+        tensor gives its layout (x, y, z[, intensity]), any other needs `layout` (a PwppPointLayout), and the buffer holds
+        nbytes // point_step records. `offsets`: a contiguous int64 CUDA tensor of nframes + 1 entries. Frame f holds up to
+        max_n[f] records. `streams` and `actions` as for bind_call. The tensors are kept alive while the call is bound; the
+        offsets and the records may change between runs."""
+        import torch
+        nf = len(max_n)
+        if not (isinstance(points, torch.Tensor) and points.is_cuda and points.is_contiguous()):
+            raise PwppError("points must be a contiguous CUDA tensor")
+        if not (isinstance(offsets, torch.Tensor) and offsets.is_cuda and offsets.dtype == torch.int64 and offsets.is_contiguous()
+                and offsets.numel() == nf + 1):
+            raise PwppError(f"offsets must be a contiguous int64 CUDA tensor of {nf + 1} entries")
+        if actions is not None and not (isinstance(actions, torch.Tensor) and actions.is_cuda and actions.dtype == torch.int32
+                                        and actions.is_contiguous() and actions.numel() == nf):
+            raise PwppError(f"actions must be a contiguous int32 CUDA tensor of {nf} entries")
+        if layout is None:
+            if points.dtype != torch.float32 or points.dim() != 2 or points.shape[1] not in (3, 4):
+                raise PwppError("points needs a layout unless it is a float32 (N, 4) or (N, 3) tensor")
+            cols = int(points.shape[1])
+            layout = layout_from_dtype(np.dtype({"names": ["x", "y", "z", "intensity"][:cols], "formats": ["<f4"] * cols,
+                                                 "offsets": [0, 4, 8, 12][:cols], "itemsize": 4 * cols}))
+        capacity = points.numel() * points.element_size() // layout.point_step if layout.point_step > 0 else 0
+        ids = np.arange(nf, dtype=np.int32) if streams is None else self._stream_table(streams, nf)
+        n = (C.c_int64 * max(nf, 1))(*[int(k) for k in max_n])
+        _check(self.lib.pwpp_bind_call_packed(self._h, nf, ids.ctypes.data, C.c_void_p(points.data_ptr()), C.byref(layout), capacity, n,
+                                              C.c_void_p(offsets.data_ptr()), C.c_void_p(actions.data_ptr() if actions is not None else None)))
+        self._bound = ([points] * nf, offsets, ids.tolist(), sum(int(k) for k in max_n))
+        self._bound_actions = actions
+
+    def bind_packed_xyz(self, ground: bool = True, nonground: bool = True):
+        """Enables packed xyz results for the bound call (pwpp_bind_packed_xyz): every later run_bound_call, and every graph
+        captured after this, also writes each part's xyz rows of all frames back to back and their device offsets. Host work
+        that synchronizes: call it before a capture."""
+        _check(self.lib.pwpp_bind_packed_xyz(self._h, (1 if ground else 0) | (2 if nonground else 0)))
+
+    def bound_packed_xyz(self):
+        """Zero-copy views of the packed xyz results (pwpp_bound_packed_xyz), as a dict: ground / nonground float32 CUDA tensors
+        (sum(max_n), 3) and ground_offsets / nonground_offsets int64 CUDA tensors (nframes + 1,), None for a part that is not
+        enabled. After a run or replay frame f's non-ground cloud is nonground[nonground_offsets[f]:nonground_offsets[f + 1]].
+        Fixed addresses while the call is bound."""
+        import torch
+        ptrs = [C.c_void_p() for _ in range(4)]
+        _check(self.lib.pwpp_bound_packed_xyz(self._h, *[C.byref(p) for p in ptrs]))
+        nf, rows = len(self._bound[0]), self._bound[3]
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr, shape, typestr):
+                self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (ptr, False), "version": 3, "strides": None}
+
+        def view(ptr, shape, typestr):
+            if not ptr:
+                return None
+            if 0 in shape:
+                return torch.empty(shape, dtype=torch.float32, device="cuda")
+            return torch.as_tensor(_View(ptr, shape, typestr), device="cuda")
+        g, n, go, no = (p.value for p in ptrs)
+        return {"ground": view(g, (rows, 3), "<f4"), "nonground": view(n, (rows, 3), "<f4"),
+                "ground_offsets": view(go, (nf + 1,), "<i8"), "nonground_offsets": view(no, (nf + 1,), "<i8")}
 
     def bound_call_slots(self):
         """Torch view (int32 [nframes]) of the slots the last run read (pwpp_bound_call_slots): the run's own copy, -1 where the
