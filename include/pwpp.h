@@ -390,8 +390,8 @@ int pwpp_bind_call_actions(pwpp_ctx* ctx, int nframes, const int32_t* streams, c
  *     d_slots holds.
  *   - Shared rings. Several frame entries may name the same ring, with identical descriptors: for example one sensor's backlog,
  *     its stream bound twice, the second entry reading the next slot or skipped.
- *   - The caller's obligation. Between a run's first kernel and the end of its last kernel (the record gather, when enabled), the
- *     caller must not write a slot the run reads (its records or its count). Writing other slots, d_slots and other slots'
+ *   - The caller's obligation. Between a run's first kernel and the end of its last kernel (the record gather or the packed
+ *     records gather, when enabled), the caller must not write a slot the run reads (its records or its count). Writing other slots, d_slots and other slots'
  *     counts is allowed and does not affect the run.
  *   - Bind-time checks, before anything is allocated, each message naming the frame (PWPP_ERR_INVALID_ARG): every check of
  *     pwpp_bind_call with frames[f] = base and n = max_n; NULL rings, d_slots or d_counts; NULL base with max_n > 0;
@@ -436,8 +436,8 @@ int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read);
  *   - What is read. No byte outside [base, base + capacity * point_step) is read, whatever d_offsets holds.
  *   - Results. Everything else is as for pwpp_bind_call_actions: the stream table and run split, the record results, the getter
  *     results, the freeze and pwpp_unbind_call. The index lists stay frame-relative (index k of frame f is record lo + k).
- *   - The caller's obligation. Between a run's first kernel and the end of its last kernel, the caller must not write the offsets
- *     or the records of the frames the run reads.
+ *   - The caller's obligation. Between a run's first kernel and the end of its last kernel (the packed records gather, when
+ *     enabled), the caller must not write the offsets or the records of the frames the run reads.
  *   - Bind-time checks, before anything is allocated, each message naming the frame or the field (PWPP_ERR_INVALID_ARG or
  *     PWPP_ERR_UNSUPPORTED): every check of pwpp_bind_call with frames[f] = base, layouts[f] = *layout and n = max_n[f]; NULL
  *     layout or d_offsets; NULL base with capacity > 0; capacity < 0; capacity * point_step or its end address overflowing.
@@ -464,11 +464,41 @@ int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read);
  *     invalid count, slot or offsets have count 0. Rows past off[nframes] are never written.
  *   - Independent of the getter results: both can be enabled, and each writes its own buffers.
  *   - pwpp_launch_count rises, per pwpp_run_bound_call, by two launches after the last run's output kernel (the offset scan and
- *     the gather), also when every max_n is 0.
+ *     the gather), also when every max_n is 0. The offset scan is shared with packed records (below).
  *   - Memory: 12 sum(max_n) bytes per enabled part plus 16 (nframes + 1) bytes of offsets.
  *
  * pwpp_bound_packed_xyz: host-only. The fixed device pointers of both buffers and both offsets arrays (NULL for a part that is
- * not enabled). PWPP_ERR_INVALID_ARG when no call is bound or packed xyz is not enabled. */
+ * not enabled). PWPP_ERR_INVALID_ARG when no call is bound or packed xyz is not enabled.
+ *
+ * Packed records of a bound call: the ground and non-ground clouds in the sensor's own record layout (every field, byte for
+ * byte, as pwpp_bind_record_results writes them) with all frames back to back and device offsets, for a consumer that takes one
+ * packed batch: a detector's (N, 4) xyzi batch with its batch offsets, a multi-sweep stage that needs each point's time, one
+ * merged cloud published in the drivers' own layout.
+ *
+ * pwpp_bind_packed_records: enables them for any bound call (plain, with actions, rings or packed). parts is PWPP_PART_GROUND,
+ * PWPP_PART_NONGROUND or both (3). Host work that synchronizes, so it is not capturable; graphs captured before it do not write
+ * these results. PWPP_ERR_INVALID_ARG when no call is bound, for parts outside {1, 2, 3}, and when packed records are already
+ * enabled (one setting per bind: pwpp_unbind_call releases the buffers). Every frame of the bound call must have the same
+ * point_step, so that a part is one (rows, point_step) byte array (field offsets and datatypes may differ: the bytes are copied
+ * as they are); otherwise PWPP_ERR_UNSUPPORTED, the message naming the first frame whose point_step differs from frame 0's.
+ * Such a call keeps the capacity layout of pwpp_bind_record_results. The buffers are not work buffers: the freeze does not apply.
+ *   - Layout. Per enabled part, one buffer of sum(max_n) records of point_step bytes and a device int64[nframes + 1] offsets array
+ *     in records. After every run or replay frame f's records of a part are records [off[f], off[f + 1]) of that part's buffer,
+ *     at byte off[f] * point_step, with no padding: neighbouring frames may share a 16-byte word. Record k of a frame is record k
+ *     of its list in the order the call was bound with, byte for byte what pwpp_bind_record_results writes for the frame after
+ *     the same run. Skipped frames and frames with an invalid count, slot or offsets have count 0. No byte at or past
+ *     off[nframes] * point_step is written.
+ *   - The offsets are packed xyz's: when both are enabled, pwpp_bound_packed_xyz and pwpp_bound_packed_records return the same
+ *     two arrays, filled by one scan per run. The scan writes both arrays whichever parts are enabled.
+ *   - pwpp_launch_count rises, per pwpp_run_bound_call, after the last run's output kernel, by one offset scan when packed xyz
+ *     or packed records is enabled (one, not two, when both are) plus one gather per enabled feature, also when every max_n is 0.
+ *   - The caller's obligation. The gather reads the caller's records, as the record results' gather does: the records a run
+ *     reads stay unwritten until the end of this gather.
+ *   - Direct calls between runs never write these buffers.
+ *   - Memory: point_step sum(max_n) bytes per enabled part, plus 16 (nframes + 1) bytes of offsets unless packed xyz is enabled.
+ *
+ * pwpp_bound_packed_records: host-only. The fixed device pointers of both buffers and both offsets arrays (NULL for a part that
+ * is not enabled) and the common point_step. PWPP_ERR_INVALID_ARG when no call is bound or packed records are not enabled. */
 #define PWPP_OFFSETS_OUT_OF_RANGE 5   /* d_status[f]: d_offsets[f], d_offsets[f + 1] not 0 <= lo <= hi <= capacity; empty frame */
 int pwpp_bind_call_packed(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* base, const pwpp_point_layout* layout,
                           int64_t capacity /* records at base */, const int64_t* max_n, const int64_t* d_offsets /* device [nframes + 1] */,
@@ -484,6 +514,9 @@ int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void**
 int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts /* PWPP_PART_* bits: 1, 2 or 3 */);
 int pwpp_bound_packed_xyz(pwpp_ctx* ctx, const float** d_ground, const float** d_nonground, const int64_t** d_ground_off,
                           const int64_t** d_nonground_off);
+int pwpp_bind_packed_records(pwpp_ctx* ctx, int parts /* PWPP_PART_* bits: 1, 2 or 3 */);
+int pwpp_bound_packed_records(pwpp_ctx* ctx, const void** d_ground, const void** d_nonground, const int64_t** d_ground_off,
+                              const int64_t** d_nonground_off, int32_t* point_step);
 
 /* Getter results of the bound call: what the reference's other getters return (getGround / getNonground, getCenters /
  * getNormals, getHeight and the adaptive thresholds, H:154-163), at fixed device addresses, for a graph whose next stage takes

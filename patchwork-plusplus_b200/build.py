@@ -116,6 +116,12 @@ def build_examples(force=False):
     if force or _newer(out10, [src10] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out10, src10])
+    # the kernels of a bound call's packed records, the same way (GPU cases of tests/test_records_packed_backends.py)
+    src11 = os.path.join(REPO, "tests", "gpu_records_packed_probe.cu")
+    out11 = os.path.join(LIB, "libpwpp_records_packed_probe.so")
+    if force or _newer(out11, [src11] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out11, src11])
     return out
 
 

@@ -277,7 +277,10 @@ struct pwpp_ctx {
     DevBuf<pwpp_state, false> d_bstates;    // [F] the state of every frame's stream right after the frame
     int packed_xyz = 0;                     // packed xyz results (pwpp_bind_packed_xyz): PWPP_PART_* bits, 0 = off
     DevBuf<float, false> d_pgxyz, d_pngxyz;  // [sum(max_n)][3] packed ground / non-ground xyz
-    DevBuf<long long, false> d_pg_off, d_png_off;   // [F+1] their row offsets, scanned on the device at every run
+    DevBuf<long long, false> d_pg_off, d_png_off;   // [F+1] ground / non-ground offsets of packed xyz and packed records, scanned
+                                                     // on the device at every run when either is enabled
+    int packed_rec = 0;                     // packed records (pwpp_bind_packed_records): PWPP_PART_* bits, 0 = off
+    DevBuf<unsigned char, false> d_prec_g, d_prec_ng;   // [sum(max_n)][point_step] packed ground / non-ground records
   } bound;
   int scratch_slots = 0;                  // state / history slots after the streams' (pwpp_bind_call_actions), kept after unbind
 
@@ -1672,12 +1675,21 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     ++ctx->launches;
     CU_TRY(cudaGetLastError());
   }
-  if (b.packed_xyz) {   // the offsets of both parts from the final counts, then the rows
+  if (b.packed_xyz || b.packed_rec) {   // the offsets of both parts from the final counts (one scan for both), then the rows
     k_bound_xyz_offsets<<<1, BT_THREADS, 0, s>>>(nf, ctx->d_pt_off.p, ctx->d_counts.p, b.d_pg_off.p, b.d_png_off.p);
-    const int first = b.packed_xyz == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.packed_xyz == 3 ? 2 : 1;
-    k_gather_xyz_packed<<<dim3((unsigned) b.xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
-        ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_pg_off.p, b.d_png_off.p, first, b.d_pgxyz.p, b.d_pngxyz.p);
-    ctx->launches += 2;
+    ++ctx->launches;
+    if (b.packed_xyz) {
+      const int first = b.packed_xyz == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.packed_xyz == 3 ? 2 : 1;
+      k_gather_xyz_packed<<<dim3((unsigned) b.xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
+          ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_pg_off.p, b.d_png_off.p, first, b.d_pgxyz.p, b.d_pngxyz.p);
+      ++ctx->launches;
+    }
+    if (b.packed_rec) {   // the records the runs read, as k_gather_record_parts reads them
+      const int first = b.packed_rec == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.packed_rec == 3 ? 2 : 1;
+      k_gather_record_packed<<<dim3((unsigned) b.rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
+          recs, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_pg_off.p, b.d_png_off.p, first, b.d_prec_g.p, b.d_prec_ng.p);
+      ++ctx->launches;
+    }
     CU_TRY(cudaGetLastError());
   }
   make_bound_last(ctx, s);
@@ -1780,6 +1792,17 @@ int pwpp_bind_getter_results(pwpp_ctx* ctx, int what) {
   return PWPP_OK;
 }
 
+// The ground and non-ground offsets that packed xyz and packed records share (k_bound_xyz_offsets writes both at every run):
+// reserved and zeroed by whichever of the two is enabled first.
+static int reserve_packed_offsets(pwpp_ctx::Bound& b) {
+  if (b.packed_xyz || b.packed_rec) return PWPP_OK;
+  CU_TRY(b.d_pg_off.reserve(b.nf + 1));
+  CU_TRY(b.d_png_off.reserve(b.nf + 1));
+  CU_TRY(cudaMemset(b.d_pg_off.p, 0, (size_t) (b.nf + 1) * sizeof(long long)));
+  CU_TRY(cudaMemset(b.d_png_off.p, 0, (size_t) (b.nf + 1) * sizeof(long long)));
+  return PWPP_OK;
+}
+
 int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   pwpp_ctx::Bound& b = ctx->bound;
@@ -1792,13 +1815,48 @@ int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts) {
   const size_t rows = (size_t) std::max<long long>(b.cap_pt_off[nf], 1);
   if (parts & PWPP_PART_GROUND) CU_TRY(b.d_pgxyz.reserve(3 * rows));
   if (parts & PWPP_PART_NONGROUND) CU_TRY(b.d_pngxyz.reserve(3 * rows));
-  CU_TRY(b.d_pg_off.reserve(nf + 1));
-  CU_TRY(b.d_png_off.reserve(nf + 1));
-  CU_TRY(cudaMemset(b.d_pg_off.p, 0, (size_t) (nf + 1) * sizeof(long long)));
-  CU_TRY(cudaMemset(b.d_png_off.p, 0, (size_t) (nf + 1) * sizeof(long long)));
+  if ((rc = reserve_packed_offsets(b))) return rc;
   CU_TRY(cudaDeviceSynchronize());
   b.xyz_gx = xyz_parts_grid_x(b.cap_pt_off.data(), nf);
   b.packed_xyz = parts;
+  return PWPP_OK;
+}
+
+int pwpp_bind_packed_records(pwpp_ctx* ctx, int parts) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
+  if (b.packed_rec) return fail(PWPP_ERR_INVALID_ARG, "packed records are already enabled for the bound call");
+  const int nf = b.nf;
+  for (int f = 1; f < nf; ++f)   // one step for the whole buffer: each part is one (rows, point_step) byte array
+    if (b.recs[f].step != b.recs[0].step)
+      return fail(PWPP_ERR_UNSUPPORTED, "frame " + std::to_string(f) + " has point_step " + std::to_string(b.recs[f].step) + ", frame 0 has " +
+                                            std::to_string(b.recs[0].step) + ": packed records need one point_step (pwpp_bind_record_results does not)");
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const size_t bytes = (size_t) std::max<long long>(b.cap_pt_off[nf], 1) * (size_t) b.recs[0].step;
+  if (parts & PWPP_PART_GROUND) CU_TRY(b.d_prec_g.reserve(bytes));
+  if (parts & PWPP_PART_NONGROUND) CU_TRY(b.d_prec_ng.reserve(bytes));
+  if ((rc = reserve_packed_offsets(b))) return rc;
+  CU_TRY(cudaDeviceSynchronize());
+  b.rec_gx = rec_parts_grid_x(b.cap_pt_off.data(), b.recs.data(), nf);
+  b.packed_rec = parts;
+  return PWPP_OK;
+}
+
+int pwpp_bound_packed_records(pwpp_ctx* ctx, const void** d_ground, const void** d_nonground, const int64_t** d_ground_off,
+                              const int64_t** d_nonground_off, int32_t* point_step) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  const pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (!b.packed_rec) return fail(PWPP_ERR_INVALID_ARG, "packed records are not enabled for the bound call (pwpp_bind_packed_records)");
+  const bool g = b.packed_rec & PWPP_PART_GROUND, n = b.packed_rec & PWPP_PART_NONGROUND;
+  if (d_ground) *d_ground = g ? b.d_prec_g.p : nullptr;
+  if (d_nonground) *d_nonground = n ? b.d_prec_ng.p : nullptr;
+  if (d_ground_off) *d_ground_off = g ? reinterpret_cast<const int64_t*>(b.d_pg_off.p) : nullptr;
+  if (d_nonground_off) *d_nonground_off = n ? reinterpret_cast<const int64_t*>(b.d_png_off.p) : nullptr;
+  if (point_step) *point_step = b.recs[0].step;
   return PWPP_OK;
 }
 

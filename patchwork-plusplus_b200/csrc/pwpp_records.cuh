@@ -587,19 +587,23 @@ __global__ void __launch_bounds__(REC_THREADS, 4) k_gather_records(const RecordF
 // (counts: the call's count rows, num_ground, num_patches, num_dropped). The grid is sized from the capacities, so CTAs past the
 // list return at once; CTA (0, f, 0) writes both counts of the frame to part_cnt[2f], part_cnt[2f + 1], whichever parts run.
 // Frame f's tiles stay inside [part_off[f], part_off[f] + count * step) and read only [src, src + n * step).
-__global__ void __launch_bounds__(REC_THREADS, 4) k_gather_record_parts(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
-                                                                      const int* __restrict__ counts, int nf, const int* __restrict__ idx,
-                                                                      const long long* __restrict__ part_off, int first,
-                                                                      unsigned char* __restrict__ ground, unsigned char* __restrict__ nonground,
-                                                                      int* __restrict__ part_cnt) {
-  __shared__ __align__(16) unsigned s_w[REC_SMEM_WORDS];
-  __shared__ int s_idx[REC_MAX_TILE_PTS];
+//
+// k_gather_record_packed (pwpp_bind_packed_records) is the same gather into packed records: every frame of the call has the
+// same step, g_off / ng_off are each part's record offsets (k_bound_xyz_offsets, in records), and frame f's list of a part goes
+// to dst_z + off_z[f] * step with no padding between frames, so neighbouring frames may share a 16-byte word (rec_gather_tile
+// writes only its own bytes). It writes no counts. Frame f's tiles stay inside [off_z[f] * step, off_z[f + 1] * step).
+template <bool Packed>
+__device__ __forceinline__ void gather_record_parts_body(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
+                                                         const int* __restrict__ counts, int nf, const int* __restrict__ idx,
+                                                         const long long* __restrict__ g_off, const long long* __restrict__ ng_off, int first,
+                                                         unsigned char* __restrict__ ground, unsigned char* __restrict__ nonground,
+                                                         int* __restrict__ part_cnt, unsigned* s_w, int* s_idx) {
   const int f = blockIdx.y, part = first + (int) blockIdx.z;
   const long long p0 = pt_off[f];
   const long long n = pt_off[f + 1] - p0;
   const int ng = counts[f];
   const long long nn = n - ng - counts[2 * nf + f];
-  if (blockIdx.x == 0 && blockIdx.z == 0 && threadIdx.x == 0) { part_cnt[2 * f] = ng; part_cnt[2 * f + 1] = (int) nn; }
+  if (!Packed && blockIdx.x == 0 && blockIdx.z == 0 && threadIdx.x == 0) { part_cnt[2 * f] = ng; part_cnt[2 * f + 1] = (int) nn; }
   const long long m = part ? nn : ng;
   const int step = recs[f].step;
   const int tp = rec_tile_pts(step);
@@ -608,7 +612,28 @@ __global__ void __launch_bounds__(REC_THREADS, 4) k_gather_record_parts(const Re
   const int cnt = (int) (m - k0 < tp ? m - k0 : tp);
   const unsigned char* lo = recs[f].src;
   unsigned char* dst = part ? nonground : ground;
-  rec_gather_tile(lo, lo + n * step, step, idx, p0 + (part ? ng : 0) + k0, cnt, dst + part_off[f] + k0 * step, s_w, s_idx);
+  const long long o = Packed ? (part ? ng_off : g_off)[f] * step : g_off[f];   // the byte offset of the frame's region
+  rec_gather_tile(lo, lo + n * step, step, idx, p0 + (part ? ng : 0) + k0, cnt, dst + o + k0 * step, s_w, s_idx);
+}
+
+__global__ void __launch_bounds__(REC_THREADS, 4) k_gather_record_parts(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
+                                                                      const int* __restrict__ counts, int nf, const int* __restrict__ idx,
+                                                                      const long long* __restrict__ part_off, int first,
+                                                                      unsigned char* __restrict__ ground, unsigned char* __restrict__ nonground,
+                                                                      int* __restrict__ part_cnt) {
+  __shared__ __align__(16) unsigned s_w[REC_SMEM_WORDS];
+  __shared__ int s_idx[REC_MAX_TILE_PTS];
+  gather_record_parts_body<false>(recs, pt_off, counts, nf, idx, part_off, part_off, first, ground, nonground, part_cnt, s_w, s_idx);
+}
+
+__global__ void __launch_bounds__(REC_THREADS, 4) k_gather_record_packed(const RecordFrame* __restrict__ recs, const long long* __restrict__ pt_off,
+                                                                       const int* __restrict__ counts, int nf, const int* __restrict__ idx,
+                                                                       const long long* __restrict__ g_off, const long long* __restrict__ ng_off,
+                                                                       int first, unsigned char* __restrict__ ground,
+                                                                       unsigned char* __restrict__ nonground) {
+  __shared__ __align__(16) unsigned s_w[REC_SMEM_WORDS];
+  __shared__ int s_idx[REC_MAX_TILE_PTS];
+  gather_record_parts_body<true>(recs, pt_off, counts, nf, idx, g_off, ng_off, first, ground, nonground, nullptr, s_w, s_idx);
 }
 
 // Byte offsets of every frame's output region (16-byte aligned, room for all n[f] records): off[nf + 1].

@@ -81,6 +81,8 @@ def load_library():
     lib.pwpp_bind_call_packed.argtypes = [vp, i32, vp, vp, C.POINTER(PwppPointLayout), i64, vp, vp, vp]; lib.pwpp_bind_call_packed.restype = i32
     lib.pwpp_bind_packed_xyz.argtypes = [vp, i32]; lib.pwpp_bind_packed_xyz.restype = i32
     lib.pwpp_bound_packed_xyz.argtypes = [vp] + [C.POINTER(vp)] * 4; lib.pwpp_bound_packed_xyz.restype = i32
+    lib.pwpp_bind_packed_records.argtypes = [vp, i32]; lib.pwpp_bind_packed_records.restype = i32
+    lib.pwpp_bound_packed_records.argtypes = [vp] + [C.POINTER(vp)] * 4 + [C.POINTER(i32)]; lib.pwpp_bound_packed_records.restype = i32
     lib.pwpp_run_bound_call.argtypes = [vp, vp]; lib.pwpp_run_bound_call.restype = i32
     lib.pwpp_bound_call_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_bound_call_results.restype = i32
     lib.pwpp_unbind_call.argtypes = [vp]; lib.pwpp_unbind_call.restype = i32
@@ -430,6 +432,41 @@ class Engine:
         g, n, go, no = (p.value for p in ptrs)
         return {"ground": view(g, (rows, 3), "<f4"), "nonground": view(n, (rows, 3), "<f4"),
                 "ground_offsets": view(go, (nf + 1,), "<i8"), "nonground_offsets": view(no, (nf + 1,), "<i8")}
+
+    def bind_packed_records(self, ground: bool = True, nonground: bool = True):
+        """Enables packed records for the bound call (pwpp_bind_packed_records): every later run_bound_call, and every graph
+        captured after this, also writes each part's records of all frames back to back, in the sensor's own layout, and their
+        device offsets. Every frame of the call must have the same point_step. Host work that synchronizes: call it before a
+        capture."""
+        _check(self.lib.pwpp_bind_packed_records(self._h, (1 if ground else 0) | (2 if nonground else 0)))
+
+    def bound_packed_records(self):
+        """Zero-copy views of the packed records (pwpp_bound_packed_records), as a dict: ground / nonground uint8 CUDA tensors
+        (sum(max_n), point_step) and ground_offsets / nonground_offsets int64 CUDA tensors (nframes + 1,), None for a part that
+        is not enabled, and point_step. After a run or replay frame f's non-ground records are
+        nonground[nonground_offsets[f]:nonground_offsets[f + 1]]. For a 16-byte float32 layout (x, y, z, intensity),
+        nonground.view(torch.float32) is the (sum(max_n), 4) xyzi batch and nonground_offsets its batch offsets. The offsets are
+        those of bound_packed_xyz when both are enabled. Fixed addresses while the call is bound."""
+        import torch
+        ptrs = [C.c_void_p() for _ in range(4)]
+        step = C.c_int32()
+        _check(self.lib.pwpp_bound_packed_records(self._h, *[C.byref(p) for p in ptrs], C.byref(step)))
+        nf, rows, step = len(self._bound[0]), self._bound[3], step.value
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr, shape, typestr):
+                self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (ptr, False), "version": 3, "strides": None}
+
+        def view(ptr, shape, typestr, dtype):
+            if not ptr:
+                return None
+            if 0 in shape:
+                return torch.empty(shape, dtype=dtype, device="cuda")
+            return torch.as_tensor(_View(ptr, shape, typestr), device="cuda")
+        g, n, go, no = (p.value for p in ptrs)
+        return {"ground": view(g, (rows, step), "|u1", torch.uint8), "nonground": view(n, (rows, step), "|u1", torch.uint8),
+                "ground_offsets": view(go, (nf + 1,), "<i8", torch.int64), "nonground_offsets": view(no, (nf + 1,), "<i8", torch.int64),
+                "point_step": step}
 
     def bound_call_slots(self):
         """Torch view (int32 [nframes]) of the slots the last run read (pwpp_bound_call_slots): the run's own copy, -1 where the
