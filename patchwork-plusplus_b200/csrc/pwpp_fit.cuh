@@ -442,9 +442,12 @@ __device__ __forceinline__ int dist_filter(const PlaneF& pf, float th, float x, 
 // cross-warp prefix. The LPR selection is two-level: the num_lpr-th smallest of the 256 per-thread minima bounds
 // the num_lpr-th smallest point from above, so only the few points not above that bound are gathered and
 // selected exactly by one warp.
-// PLS (PWPP_L2_PLS): the current plane lives in shared memory (s_plane) instead of 20 registers per thread — warp 0 rewrites it
-// in place between the two barriers of a round, when no other warp reads it — so that the fused kernel fits the 64-register
-// budget of 4 CTAs per SM with far fewer spills.
+// PLS (class L2): state that is not per point stays out of registers, so that the fused kernel comes close to the 64-register
+// budget of 4 CTAs per SM. The current plane lives in shared memory (s_plane) — warp 0 rewrites it in place between the two
+// barriers of a round, when no other warp reads it —, and so do the running sums of the R-GPF phase (s_tot: lane q of warp 0
+// keeps quantity q), the look-ahead descriptor (s_next) and the reference point (the staged first point and s_lpr). A fused
+// round sums its inner seed set in a second pass over the points, so one set of nine sums is live at a time; the per-thread
+// partials are the same, so the results are bit-identical to the one-pass form.
 template <int CAP, int CLS, int MINB, int NW, bool FUSE = false, bool PLS = false>
 __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states,
                                                                                 const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps, int nbp, const int* __restrict__ bin_off, WorkQueues wq,
@@ -471,6 +474,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
   __shared__ int s_ccount, s_mn, s_fix, s_refit;
   __shared__ int4 s_item;
   __shared__ Plane s_plane;
+  __shared__ double s_tot[PLS ? 9 : 1];
+  __shared__ int s_totn;
+  __shared__ int4 s_next;
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int count = wq.count[CLS];
   const int4 no_item = make_int4(-1, 0, 0, 0);
@@ -510,6 +516,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
     if (w == LOOK_W) {
       const int t = __shfl_sync(0xffffffffu, next_raw, 0);
       if (t < count) nxt = wq.items[CLS][t];
+      if (PLS && lane == 0) s_next = nxt;
     }
     unsigned amask = vmask;
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
@@ -668,7 +675,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         const double lpr = s_lpr;
         zthr = float_ru(lpr + (state == ST_RVPF ? ap.th_seeds_v : ap.th_seeds));
         zin = float_ru(lpr + ap.th_seeds);
-        c[0] = c0x; c[1] = c0y; c[2] = lpr;
+        c[0] = PLS ? (double) sx[0] : c0x; c[1] = PLS ? (double) sy[0] : c0y; c[2] = lpr;
       }
       // ---- predicate + moments ----
       // Seed rounds accumulate their whole set. R-GPF rounds are incremental (see k_fit_warp): every fit of the
@@ -676,7 +683,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
       // the points whose membership changed, warp 0 keeps the running sums, and a round without any change is the
       // fixpoint of S:516-543.
       const bool incr = !seed_round;
-      if (incr) { c[0] = c0x; c[1] = c0y; c[2] = c_lpr; }
+      if (incr) { c[0] = PLS ? (double) sx[0] : c0x; c[1] = PLS ? (double) sy[0] : c0y; c[2] = PLS ? s_lpr : c_lpr; }
       else if (state == ST_SEED || (FUSE && fused)) c_lpr = c[2];
       PlaneF pf;
       pf.n0 = (float) pl.normal[0]; pf.n1 = (float) pl.normal[1]; pf.n2 = (float) pl.normal[2]; pf.d = (float) pl.d;
@@ -713,6 +720,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         mn += in ? 1 : -1;
         if (FUSE && fused && (z < zin)) {   // also a seed of the R-GPF seed fit (in is true here)
           seli |= 1u << it;
+          if (PLS) continue;
           bi[0] += dx; bi[1] += dy; bi[2] += dz;
           bi[3] += dx * dx; bi[4] += dx * dy; bi[5] += dx * dz; bi[6] += dy * dy; bi[7] += dy * dz; bi[8] += dz * dz;
           ++mni;
@@ -724,7 +732,27 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
       const int buf = round & 1;
       ++round;
       // warp sums by reduce-scatter: the lane that ends up holding quantity q stores it
-      if (FUSE && fused) {
+      if (PLS && FUSE && fused) {   // the inner set in a second pass, so that one set of sums is live at a time
+        reduce_scatter<9, 16>(a, lane);
+#pragma unroll
+        for (int q = 0; q < 9; ++q)
+          if (lane == rs_lane(9, 16, q)) s_part[buf][w][q] = a[rs_slot(9, 16, q)];
+#pragma unroll
+        for (int q = 0; q < 9; ++q) a[q] = 0.0;
+        for (int it = 0; it < nit; ++it) {
+          if (!((seli >> it) & 1u)) continue;
+          const int j = jbase + it * 32;
+          const double dx = (double) sx[j] - c[0], dy = (double) sy[j] - c[1], dz = (double) sz[j] - c[2];
+          a[0] += dx; a[1] += dy; a[2] += dz;
+          a[3] += dx * dx; a[4] += dx * dy; a[5] += dx * dz; a[6] += dy * dy; a[7] += dy * dz; a[8] += dz * dz;
+        }
+        reduce_scatter<9, 16>(a, lane);
+#pragma unroll
+        for (int q = 0; q < 9; ++q)
+          if (lane == rs_lane(9, 16, q)) s_parti[FUSE ? buf : 0][FUSE ? w : 0][q] = a[rs_slot(9, 16, q)];
+        mni = __reduce_add_sync(0xffffffffu, __popc(seli));
+        if (lane == 0) s_cnt[w][1] = mni;
+      } else if (FUSE && fused) {
         double v[18];
 #pragma unroll
         for (int q = 0; q < 9; ++q) { v[q] = a[q]; v[9 + q] = bi[FUSE ? q : 0]; }
@@ -777,7 +805,10 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
           const double vz = __shfl_sync(0xffffffffu, mine.normal[2], 0);
           const bool hv = have_plane || mv.n > 0;
           const bool taken = !(hv && (mv.n > 0 ? vz : pl.normal[2]) < ap.uprightness_thr);   // S:489 false -> S:506 break
-          if (taken) tot = mi; else tot = mv;
+          if (PLS) {
+            if ((taken ? hi : !hi) && ql < 9) s_tot[PLS ? ql : 0] = v;
+            if ((taken ? hi : !hi) && ql == 9) s_totn = cn;
+          } else if (taken) tot = mi; else tot = mv;
           if (PLS) {   // the plane the next round uses goes straight to s_plane: the seed plane when taken and fitted, else the R-VPF plane
             const bool seed_wins = taken && mi.n > 0;
             if (lane == 0) { if (!seed_wins && mv.n > 0) s_plane = mine; s_mn = mv.n; s_refit = mv.n > 0 ? 1 : 0; s_fix = 0; s_taken = taken ? 1 : 0; }
@@ -787,7 +818,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
             if (lane == 16) { s_plane2 = mine; s_mni = mi.n; }
           }
         } else if (w == LOOK_W && rvpf_it == 0) {
-          if (nxt.x >= 0) prefetch_patch_l2(sorted + work_item_start(nxt), nxt.y, lane, 32);
+          const int4 nx = PLS ? s_next : nxt;
+          if (nx.x >= 0) prefetch_patch_l2(sorted + work_item_start(nx), nx.y, lane, 32);
         }
       } else
       if (w == 0) {
@@ -803,6 +835,13 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
 #pragma unroll
           for (int ww = 0; ww < NW; ++ww) cn += s_pchg[buf][ww];
         }
+        if (PLS) {   // lane q < 9 keeps quantity q of the running sums, lane 9 their count
+          const int chg = __shfl_sync(0xffffffffu, cn, 10);
+          if (incr && lane < 9) { if (chg != 0) v = s_tot[PLS ? lane : 0] + v; else v = s_tot[PLS ? lane : 0]; }
+          if (incr && lane == 9) { if (chg != 0) cn = s_totn + cn; else cn = s_totn; }
+          if (lane < 9) s_tot[PLS ? lane : 0] = v;
+          if (lane == 9) s_totn = cn;
+        }
         Moments m;
 #pragma unroll
         for (int q = 0; q < 3; ++q) m.s1[q] = __shfl_sync(0xffffffffu, v, q);
@@ -811,7 +850,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         m.n = __shfl_sync(0xffffffffu, cn, 9);
         const int changed = __shfl_sync(0xffffffffu, cn, 10);
         bool refit = true;
-        if (incr) {
+        if (PLS) { if (incr && changed == 0) refit = false; tot = m; }
+        else if (incr) {
           if (changed == 0) refit = false;   // fixpoint
           else {
 #pragma unroll
@@ -828,7 +868,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         }
         if (lane == 0) { s_mn = tot.n; s_fix = (incr && changed == 0) ? 1 : 0; s_refit = (refit && tot.n > 0) ? 1 : 0; }
       } else if (w == LOOK_W && state == ST_SEED) {   // the R-GPF seed round: exactly once per patch
-        if (nxt.x >= 0) prefetch_patch_l2(sorted + work_item_start(nxt), nxt.y, lane, 32);
+        const int4 nx = PLS ? s_next : nxt;
+        if (nx.x >= 0) prefetch_patch_l2(sorted + work_item_start(nx), nx.y, lane, 32);
       }
       __syncthreads();
       int tot_n = s_mn;
@@ -864,8 +905,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
       } else {   // ST_FINAL
         state = ST_DONE;
       }
-      if (state == ST_DONE) { gmask = have_plane ? member : 0u; n_ground = have_plane ? tot_n : 0; }
+      if (!PLS && state == ST_DONE) { gmask = have_plane ? member : 0u; n_ground = have_plane ? tot_n : 0; }
     }
+    if (PLS) { gmask = have_plane ? member : 0u; n_ground = have_plane ? s_mn : 0; }
 
     // ---- stable partition: ground indices ascending, then non-ground indices ascending ----
     {
@@ -905,7 +947,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) k_fit_cta(const float4* __restr
         for (int q = 0; q < 3; ++q) { r.mean[q] = pl.mean[q]; r.normal[q] = pl.normal[q]; r.sv[q] = pl.sv[q]; }
         r.d = pl.d;
       }
-      if (tid == LOOK_TID) s_item = nxt;   // every thread read the current descriptor before the barrier above
+      if (tid == LOOK_TID) s_item = PLS ? s_next : nxt;   // every thread read the current descriptor before the barrier above
     }
     __syncthreads();
   }
