@@ -76,6 +76,9 @@ struct Params {
   std::vector<double> flatness_thr{0, 0, 0, 0};
 };
 
+// order inside a bin of the index lists (PatchWorkpp::setOutputOrder; the values are pwpp.h's PWPP_ORDER_*)
+enum class OutputOrder : int { Bin = PWPP_ORDER_BIN, Reference = PWPP_ORDER_REFERENCE, ReferenceExact = PWPP_ORDER_REFERENCE_EXACT };
+
 class PatchWorkpp {
  public:
   // reference :120-150. `device` selects the CUDA device (extension; defaults to 0).
@@ -198,6 +201,10 @@ class PatchWorkpp {
   // true (default): index lists in the reference's order inside every bin (ascending z, R-VPF removals first in the
   // non-ground part); false: ascending point index inside a bin (no sorting pass)
   void setReferenceOrder(bool on) { check(pwpp_set_output_order(ctx_, on ? PWPP_ORDER_REFERENCE : PWPP_ORDER_BIN)); }
+  // Bin: ascending point index inside a bin; Reference (default): the reference's order, equal z in ascending point index;
+  // ReferenceExact: the reference's order with equal z where libstdc++'s std::sort leaves them, so the lists equal the
+  // unmodified reference's whenever the label sets do (pwpp.h, PWPP_ORDER_REFERENCE_EXACT)
+  void setOutputOrder(OutputOrder order) { check(pwpp_set_output_order(ctx_, static_cast<int>(order))); }
 
   pwpp_ctx* handle() { return ctx_; }
 

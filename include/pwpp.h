@@ -618,10 +618,22 @@ int pwpp_device_results(pwpp_ctx* ctx, const int32_t** d_indices, const int32_t*
  *                         each in ascending z, then the final rejects in ascending z (S:199, S:495-504, S:529-541); equal z
  *                         in ascending point index (= the reference with a stable per-bin sort). One extra kernel (a sort of
  *                         every fitted patch). The drop-in C++ class and pypatchworkpp select it by default.
- * Takes effect with the next estimate call. */
+ *   PWPP_ORDER_REFERENCE_EXACT  the unmodified reference's lists: as PWPP_ORDER_REFERENCE, with equal z in the order the
+ *                         reference's std::sort leaves them as built by libstdc++ (GCC's introsort; not libc++'s or MSVC's).
+ *                         Whenever the label sets are identical to the reference's, the lists are identical element for
+ *                         element. A fix-up kernel per patch-size class runs after the sort: pwpp_launch_count rises by five
+ *                         per launch range over PWPP_ORDER_REFERENCE (one per class, on that class's stream); patches without
+ *                         two equal z in one part leave it at once. Patches above 512 points use a scratch of 16 bytes per
+ *                         point of the call, reserved with the work buffers (so a bound call reserves it at bind).
+ * Takes effect with the next estimate call. A bound call keeps the order it was bound with. */
 #define PWPP_ORDER_BIN 0
 #define PWPP_ORDER_REFERENCE 1
+#define PWPP_ORDER_REFERENCE_EXACT 2
 int pwpp_set_output_order(pwpp_ctx* ctx, int order);
+/* Counters of the PWPP_ORDER_REFERENCE_EXACT fix-up since the context was created or the last reset: out[0] = patches with a
+ * tie in z inside one part (their libstdc++ order simulated), out[1] = segments sorted by the depth-limit heap sort, out[2] =
+ * bins holding a NaN z (std::sort run literally in one thread). Synchronises the device; reset != 0 zeroes them afterwards. */
+int pwpp_order_exact_counts(pwpp_ctx* ctx, uint64_t out[3], int reset);
 
 /* Host-side zero-copy view of the index lists of the last call (batch consumers: the per-frame getters above copy each
  * list once more, which for a 1024-frame batch is 0.5 GB of host memcpy): *h_indices -> the page-locked int32 buffer the

@@ -122,6 +122,12 @@ def build_examples(force=False):
     if force or _newer(out11, [src11] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out11, src11])
+    # the reference-order sort and its libstdc++ tie fix-up alone, the same way (GPU cases of tests/test_order_exact_backends.py)
+    src12 = os.path.join(REPO, "tests", "gpu_order_exact_probe.cu")
+    out12 = os.path.join(LIB, "libpwpp_order_exact_probe.so")
+    if force or _newer(out12, [src12] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out12, src12])
     return out
 
 

@@ -186,13 +186,16 @@ struct pwpp_ctx {
   DevBuf<BinFit> d_fits;          // [F][nbins]
   DevBuf<BinSeg> d_segs;          // [F][nbins+3]
   DevBuf<int4> d_wq_items[NUM_CLASSES];  // fit work queues
-  DevBuf<int> d_wq_ctr;           // [2*NUM_CLASSES + ORD_NUM_HEADS]: counts, heads, the heads of the five k_order launches
+  DevBuf<int> d_wq_ctr;           // [2*NUM_CLASSES + 2*ORD_NUM_HEADS]: counts, heads, the heads of the five k_order and five k_order_exact launches
   DevBuf<unsigned char> d_labels; // reference-order output only: what became of every point of a fitted patch
+  DevBuf<unsigned> d_ox_scratch;  // PWPP_ORDER_REFERENCE_EXACT only: workspace of the fix-up above 512 points, OX_X_WORDS words per point
+  DevBuf<unsigned long long> d_ox_counts;   // [OX_NUM_STATS] counters of the fix-up (pwpp_order_exact_counts)
   int order_mode = 0;             // PWPP_ORDER_*
   FitLaunch fit[NUM_CLASSES];   // persistent fit kernel of every patch-size class (variant chosen in pwpp_create)
   FitLaunch fit_small[NUM_CLASSES];   // the same for calls of at most small_call_frames frames (one CTA per patch above 512 points)
   int max_sectors = 0;
   FitLaunch order_k[ORD_NUM_HEADS];   // k_order_cta<512, X>, <512, L3>, <256, L2>, <128, L1>, k_order_warp (same argument list as the fit kernels' type is not needed: launched by name)
+  FitLaunch exact_k[ORD_NUM_HEADS];   // k_order_exact_big<X>, <L3>, <L2>, <L1>, k_order_exact_warp: grid, threads and shared memory of each
   DevBuf<int> d_out_idx;
   DevBuf<int> d_counts;           // [3][F]: num_ground, num_patches, num_dropped (F = frames of the call)
   DevBuf<float> d_centers, d_normals;  // [F][nbins][3]
@@ -380,6 +383,7 @@ int reserve_work(pwpp_ctx* ctx, int nframes, long long total, long long total_ch
   need(ctx->d_sorted, np);
   need(ctx->d_part, np);
   if (ctx->order_mode) need(ctx->d_labels, np);
+  if (ctx->order_mode == PWPP_ORDER_REFERENCE_EXACT) need(ctx->d_ox_scratch, (size_t) OX_X_WORDS * std::max<size_t>(np, 1));
   need(ctx->d_fits, nf * nb);
   need(ctx->d_segs, nf * nb_all);
   for (int c = 0; c < NUM_CLASSES; ++c) need(ctx->d_wq_items[c], nf * nb);
@@ -490,7 +494,7 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
   BinSeg* segs = ctx->d_segs.p + (size_t) f0 * nb_all;
   float* centers = ctx->d_centers.p + (size_t) f0 * nb * 3;
   float* normals = ctx->d_normals.p + (size_t) f0 * nb * 3;
-  CU_TRY(cudaMemsetAsync(ctx->d_wq_ctr.p, 0, (2 * NUM_CLASSES + ORD_NUM_HEADS) * sizeof(int), s));
+  CU_TRY(cudaMemsetAsync(ctx->d_wq_ctr.p, 0, (2 * NUM_CLASSES + 2 * ORD_NUM_HEADS) * sizeof(int), s));
   int stage = 0;
 #define STAGE_MARK() do { if (prof) CU_TRY(cudaEventRecord(ctx->stage_ev[stage], s)); ++stage; } while (0)
   STAGE_MARK();
@@ -581,6 +585,22 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
       case 2: k_order_cta<256, 3><<<grid, th, sm, so>>>(ctx->d_sorted.p, wq, heads + q, ctx->d_part.p); break;
       case 3: k_order_cta<128, 2><<<grid, th, sm, so>>>(ctx->d_sorted.p, wq, heads + q, ctx->d_part.p); break;
       default: k_order_warp<<<grid, th, 0, so>>>(ctx->d_sorted.p, wq, heads + q, ctx->d_part.p); break;
+    }
+    ++ctx->launches;
+    if (ctx->order_mode != PWPP_ORDER_REFERENCE_EXACT) return;
+    // the libstdc++ order of equal z (pwpp_order_exact.cuh): behind the class's sort, on the same stream, its own ticket counter
+    const int gx = (int) std::min<long long>(ctx->exact_k[q].grid, std::max<long long>(1, (long long) nframes * (q == 4 ? 64 : 32)));
+    const int tx = ctx->exact_k[q].threads;
+    const size_t smx = ctx->exact_k[q].smem;
+    int* hx = heads + ORD_NUM_HEADS + q;
+    unsigned* xws = ctx->d_ox_scratch.p;
+    unsigned long long* cnt = ctx->d_ox_counts.p;
+    switch (q) {
+      case 0: k_order_exact_big<5><<<gx, tx, smx, so>>>(ctx->d_sorted.p, wq, hx, ctx->d_part.p, xws, cnt); break;
+      case 1: k_order_exact_big<4><<<gx, tx, smx, so>>>(ctx->d_sorted.p, wq, hx, ctx->d_part.p, xws, cnt); break;
+      case 2: k_order_exact_big<3><<<gx, tx, smx, so>>>(ctx->d_sorted.p, wq, hx, ctx->d_part.p, xws, cnt); break;
+      case 3: k_order_exact_big<2><<<gx, tx, smx, so>>>(ctx->d_sorted.p, wq, hx, ctx->d_part.p, xws, cnt); break;
+      default: k_order_exact_warp<<<gx, tx, smx, so>>>(ctx->d_sorted.p, wq, hx, ctx->d_part.p, cnt); break;
     }
     ++ctx->launches;
   };
@@ -1002,7 +1022,9 @@ static int create_impl(const pwpp_params* sets, int num_sets, const int32_t* str
   // blob holds no bytes of whatever the allocation held before
   CU_TRY_CTX(cudaMemset(ctx->d_hist.p, 0, (size_t) num_streams * 2 * 4 * ctx->hist_stride * sizeof(double)));
   CU_TRY_CTX(ctx->d_counts.reserve((size_t) 3 * num_streams));
-  CU_TRY_CTX(ctx->d_wq_ctr.reserve(2 * NUM_CLASSES + ORD_NUM_HEADS));
+  CU_TRY_CTX(ctx->d_wq_ctr.reserve(2 * NUM_CLASSES + 2 * ORD_NUM_HEADS));
+  CU_TRY_CTX(ctx->d_ox_counts.reserve(OX_NUM_STATS));
+  CU_TRY_CTX(cudaMemset(ctx->d_ox_counts.p, 0, OX_NUM_STATS * sizeof(unsigned long long)));
   {
     cudaDeviceProp prop;
     CU_TRY_CTX(cudaGetDeviceProperties(&prop, device));
@@ -1051,6 +1073,21 @@ static int create_impl(const pwpp_params* sets, int num_sets, const int32_t* str
         ctx->order_k[q].grid = std::max(1, per_sm) * prop.multiProcessorCount;
         ctx->order_k[q].threads = th[q];
         ctx->order_k[q].smem = sm;
+      }
+      typedef void (*OxKernel)(const float4*, WorkQueues, int*, int*, unsigned*, unsigned long long*);
+      const OxKernel fx[4] = {k_order_exact_big<5>, k_order_exact_big<4>, k_order_exact_big<3>, k_order_exact_big<2>};
+      for (int q = 0; q < ORD_NUM_HEADS; ++q) {
+        const size_t sm = q < 4 ? 0 : ox_warp_smem_bytes();
+        int per_sm = 1;
+        if (q < 4) {
+          CU_TRY_CTX(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fx[q], OX_WARP_THREADS, 0));
+        } else {
+          if (sm > 48 * 1024) CU_TRY_CTX(raise_smem_limit(k_order_exact_warp, sm));
+          CU_TRY_CTX(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_order_exact_warp, OX_WARP_THREADS, sm));
+        }
+        ctx->exact_k[q].grid = std::max(1, per_sm) * prop.multiProcessorCount;
+        ctx->exact_k[q].threads = OX_WARP_THREADS;
+        ctx->exact_k[q].smem = sm;
       }
     }
     const size_t gle_smem = gle_smem_bytes(max_sectors);
@@ -2147,10 +2184,22 @@ int pwpp_device_results(pwpp_ctx* ctx, const int32_t** d_indices, const int32_t*
 
 int pwpp_set_output_order(pwpp_ctx* ctx, int order) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  if (order != PWPP_ORDER_BIN && order != PWPP_ORDER_REFERENCE) return fail(PWPP_ERR_INVALID_ARG, "order must be PWPP_ORDER_BIN or PWPP_ORDER_REFERENCE");
+  if (order != PWPP_ORDER_BIN && order != PWPP_ORDER_REFERENCE && order != PWPP_ORDER_REFERENCE_EXACT)
+    return fail(PWPP_ERR_INVALID_ARG, "order must be PWPP_ORDER_BIN, PWPP_ORDER_REFERENCE or PWPP_ORDER_REFERENCE_EXACT");
   if (ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "the output order cannot change while a call is bound (it keeps the order it was bound with)");
   if (order != ctx->order_mode) ++g_alloc_gen;   // captured graphs were recorded with the other launch sequence
   ctx->order_mode = order;
+  return PWPP_OK;
+}
+
+int pwpp_order_exact_counts(pwpp_ctx* ctx, uint64_t out[3], int reset) {
+  if (!ctx || !out) return fail(PWPP_ERR_INVALID_ARG, "ctx or out is NULL");
+  CU_TRY(cudaSetDevice(ctx->device));
+  CU_TRY(cudaDeviceSynchronize());
+  unsigned long long c[OX_NUM_STATS];
+  CU_TRY(cudaMemcpy(c, ctx->d_ox_counts.p, sizeof c, cudaMemcpyDeviceToHost));
+  for (int k = 0; k < OX_NUM_STATS; ++k) out[k] = c[k];
+  if (reset) CU_TRY(cudaMemset(ctx->d_ox_counts.p, 0, sizeof c));
   return PWPP_OK;
 }
 

@@ -25,6 +25,7 @@
 #include "pwpp_fit_big.cuh"
 #include "pwpp_fit_patch.cuh"
 #include "pwpp_order.cuh"
+#include "pwpp_order_exact.cuh"
 #include "pwpp_front.cuh"
 
 namespace pwpp {

@@ -72,6 +72,7 @@ def load_library():
     lib.pwpp_stage_name.argtypes = [i32]; lib.pwpp_stage_name.restype = C.c_char_p
     lib.pwpp_launch_count.argtypes = [vp]; lib.pwpp_launch_count.restype = i64
     lib.pwpp_set_output_order.argtypes = [vp, i32]; lib.pwpp_set_output_order.restype = i32
+    lib.pwpp_order_exact_counts.argtypes = [vp, vp, i32]; lib.pwpp_order_exact_counts.restype = i32
     lib.pwpp_host_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_host_results.restype = i32
     lib.pwpp_bind_host_to_device.argtypes = [i32]; lib.pwpp_bind_host_to_device.restype = i32
     lib.pwpp_bind_call.argtypes = [vp, i32, vp, vp, vp, vp, vp]; lib.pwpp_bind_call.restype = i32
@@ -764,11 +765,18 @@ class Engine:
         _check(self.lib.pwpp_device_results(self._h, C.byref(a), C.byref(b)))
         return a.value, b.value
 
-    ORDER_BIN, ORDER_REFERENCE = 0, 1
+    ORDER_BIN, ORDER_REFERENCE, ORDER_REFERENCE_EXACT = 0, 1, 2
 
     def set_output_order(self, order: int):
-        """ORDER_BIN (default): ascending point index inside a bin; ORDER_REFERENCE: the reference's z order (pwpp.h)."""
+        """ORDER_BIN (default): ascending point index inside a bin; ORDER_REFERENCE: the reference's z order, equal z in ascending
+        point index; ORDER_REFERENCE_EXACT: the reference's z order with equal z as libstdc++'s std::sort leaves them (pwpp.h)."""
         _check(self.lib.pwpp_set_output_order(self._h, order))
+
+    def order_exact_counts(self, reset: bool = False):
+        """Counters of the ORDER_REFERENCE_EXACT fix-up: (patches simulated, heap fall-backs, NaN bins); synchronises the device."""
+        out = np.zeros(3, np.uint64)
+        _check(self.lib.pwpp_order_exact_counts(self._h, out.ctypes.data, 1 if reset else 0))
+        return tuple(int(v) for v in out)
 
     NUM_STAGES = 11
 

@@ -137,6 +137,14 @@ PYBIND11_MODULE(pypatchworkpp, m) {
       .def("getNormals", [](patchwork::PatchWorkpp& s) { return x3(s.getNormalsVec()); })
       .def("setReferenceOrder", &patchwork::PatchWorkpp::setReferenceOrder, py::arg("on"),
            "True (default): index lists in the reference's order inside every bin; False: ascending point index inside a bin")
+      .def("setOutputOrder", [](patchwork::PatchWorkpp& s, const std::string& order) {
+        if (order == "bin") s.setOutputOrder(patchwork::OutputOrder::Bin);
+        else if (order == "reference") s.setOutputOrder(patchwork::OutputOrder::Reference);
+        else if (order == "reference_exact") s.setOutputOrder(patchwork::OutputOrder::ReferenceExact);
+        else throw py::value_error("order must be \"bin\", \"reference\" or \"reference_exact\"");
+      }, py::arg("order"),
+           "\"bin\": ascending point index inside a bin; \"reference\" (default): the reference's order, equal z in ascending point "
+           "index; \"reference_exact\": equal z where the reference's std::sort (libstdc++) leaves them")
       .def("getGroundIndicesDevice", [](py::object self) {
         auto& s = self.cast<patchwork::PatchWorkpp&>();
         const auto v = s.groundIndicesDevice();
