@@ -106,8 +106,25 @@ class PatchWorkpp {
     std::cout << "PatchWorkpp::PatchWorkpp() - INITIALIZATION COMPLETE" << std::endl;  // reference :149
   }
   ~PatchWorkpp() { if (ctx_) pwpp_destroy(ctx_); }
-  PatchWorkpp(const PatchWorkpp&) = delete;
-  PatchWorkpp& operator=(const PatchWorkpp&) = delete;
+  // Copies, like the reference's implicit ones (its members are values): the copy gets the parameters, the adaptive state
+  // (sensor height, thresholds, both histories, the plane carried for a no-plane patch) and the last frame's results, on a
+  // ctx of its own on the same device (pwpp_clone), and prints no banner. Both then continue identically. The last call's
+  // records are not carried: getGroundRecords() / getNongroundRecords() on the copy throw until it takes records itself.
+  PatchWorkpp(const PatchWorkpp& o) : params_(o.params_), n_(o.n_), ran_(o.ran_), step_(o.step_) {
+    if (o.ctx_) check(pwpp_clone(o.ctx_, -1, &ctx_));
+  }
+  // builds the copy first, so a failure leaves *this as it was
+  PatchWorkpp& operator=(const PatchWorkpp& o) {
+    if (this != &o) {
+      PatchWorkpp copy(o);
+      std::swap(params_, copy.params_);
+      std::swap(ctx_, copy.ctx_);
+      std::swap(n_, copy.n_);
+      std::swap(ran_, copy.ran_);
+      std::swap(step_, copy.step_);
+    }
+    return *this;
+  }
   PatchWorkpp(PatchWorkpp&& o) noexcept : params_(o.params_), ctx_(o.ctx_), n_(o.n_), ran_(o.ran_), step_(o.step_) { o.ctx_ = nullptr; }
 
   // reference :152 for raw buffers: element (i,c) of the N x cols cloud is data[i*row_stride + c*col_stride].

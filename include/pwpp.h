@@ -707,6 +707,69 @@ size_t pwpp_state_blob_size(const pwpp_ctx* ctx);           /* the largest over 
 size_t pwpp_stream_state_blob_size(const pwpp_ctx* ctx, int s); /* the blob of stream s (its set's hist_cap); 0 for a bad s */
 int pwpp_export_state(pwpp_ctx* ctx, int f, void* blob /* [pwpp_state_blob_size] */);
 int pwpp_import_state(pwpp_ctx* ctx, int f, const void* blob, size_t bytes);
+
+/* ---- stream state on the GPU: snapshot, restore and fork streams inside the caller's CUDA graph --------------------------
+ * pwpp_export_state / pwpp_import_state move one stream per call through host memory and synchronize. These two move any list
+ * of streams between the ctx and a device buffer of blob rows, enqueued on a CUDA stream with no host synchronization, so a
+ * graph can snapshot its streams before a tick and roll some of them back after it on a decision made on the GPU (a check
+ * that rejects a frame, a sensor fault, a replayed segment), fork a stream into another, or hand 64 sensors to another ctx.
+ *
+ * pwpp_export_states_device: for entry i of the device list d_streams (int32[n]), the complete state of stream
+ * s = d_streams[i] into row i of d_blobs, which starts at byte i * blob_stride. The row is byte for byte what
+ * pwpp_export_state writes for s (pwpp_stream_state_blob_size(ctx, s) bytes: header, state with the carried plane, the eight
+ * history rows of s's set); bytes of the row past that size are never written. d_status[i] = PWPP_STATE_OK, or
+ * PWPP_STATE_SKIPPED for s < 0 and PWPP_STATE_OUT_OF_RANGE for s >= num_streams, whose rows are not written.
+ *
+ * pwpp_import_states_device: the reverse copy, row i into stream d_streams[i], with the checks of pwpp_import_state made on the
+ * GPU. A replay cannot return an error, so every entry gets a status in d_status[i]:
+ *   - PWPP_STATE_OK: the stream now holds the row's state.
+ *   - PWPP_STATE_SKIPPED: d_streams[i] < 0; nothing is read or written. A graph decides on the GPU which streams to restore by
+ *     writing -1 into the entries it leaves alone.
+ *   - PWPP_STATE_OUT_OF_RANGE: d_streams[i] >= num_streams. Only streams [0, num_streams) are reachable, never the scratch
+ *     slots of bound calls with actions.
+ *   - PWPP_STATE_BLOB_MISMATCH: the row's header is not one pwpp_import_state accepts for that stream (magic, PWPP_ABI_VERSION,
+ *     the history capacity of the stream's set, the state size); the stream is untouched.
+ *   - PWPP_STATE_DUPLICATE: an earlier entry of the call names the same stream; the first entry wins, whatever its status.
+ *
+ * Rules, for both:
+ *   - Capturable. No host synchronization, no allocation, no host-memory copy: kernels only, enqueued on cuda_stream (NULL =
+ *     the ctx's own stream), which may be capturing. The stream ids are read on the GPU when the launch runs, so a graph
+ *     replays with the ids the list holds at that moment; each entry reads its id once.
+ *   - Ordering is the caller's, as for pwpp_run_bound_call: calls of this ctx on other streams are not waited for. The host
+ *     getters, pwpp_get_state and pwpp_export_state see a device import once the caller has synchronized cuda_stream.
+ *   - Buffer moves. A captured graph holding these calls stays valid until the ctx's state buffers move, which only a bind
+ *     with actions may do (it grows them by its scratch slots, see pwpp_bind_call_actions): bind first, then capture.
+ *   - Host checks, before anything is launched (PWPP_ERR_INVALID_ARG): n outside [0, 65535]; NULL d_streams or d_blobs with
+ *     n > 0; blob_stride below pwpp_state_blob_size(ctx) or not a multiple of 16; d_blobs not 16-byte aligned. n == 0
+ *     launches nothing. d_status may be NULL (not written).
+ *   - pwpp_launch_count rises by 1 per export and by 2 per import (a claim launch that resolves duplicates, then the copy).
+ *   - Interop. A row copied to the host is a valid pwpp_import_state blob, and a pwpp_export_state blob copied into a row is
+ *     a valid row. The blob format is the one of pwpp_export_state.
+ *   - Memory: 8 num_streams bytes on the device for every ctx (the claim table, -1 between calls, and the history capacity of
+ *     every stream). */
+#define PWPP_STATE_OK 0
+#define PWPP_STATE_SKIPPED 1         /* d_status[i]: d_streams[i] < 0; nothing read or written */
+#define PWPP_STATE_OUT_OF_RANGE 2    /* d_status[i]: d_streams[i] >= num_streams */
+#define PWPP_STATE_BLOB_MISMATCH 3   /* d_status[i]: the row's header does not fit the stream; the stream is untouched */
+#define PWPP_STATE_DUPLICATE 4       /* d_status[i]: an earlier entry of the call names the same stream */
+int pwpp_export_states_device(pwpp_ctx* ctx, int n, const int32_t* d_streams, void* d_blobs, int64_t blob_stride,
+                              int32_t* d_status /* NULL: not written */, void* cuda_stream);
+int pwpp_import_states_device(pwpp_ctx* ctx, int n, const int32_t* d_streams, const void* d_blobs, int64_t blob_stride,
+                              int32_t* d_status /* NULL: not written */, void* cuda_stream);
+
+/* A copy of a whole ctx, what `PatchWorkpp b = a;` is for the reference's value type: a new ctx on `device` (< 0: src's
+ * device) with src's parameter sets, stream->set map, num_streams, point capacity and output order, every stream's state
+ * and histories, and the results of src's last call. Every per-frame getter answers on the clone as on src (counts, index
+ * lists, xyz, centers, normals, num_patches, bin results and ids, pwpp_time_us, pwpp_device_results and pwpp_host_results on
+ * the clone's own buffers), and the next frames give bit-identical results on both.
+ *   - Host work: synchronizes src, copies device to device (cudaMemcpyPeer when device differs from src's), then synchronizes
+ *     the clone. src is not modified.
+ *   - PWPP_ERR_INVALID_ARG while src holds a bound call (pwpp_unbind_call first): a bound call's tables point at the caller's
+ *     buffers and at graphs, which a copy cannot take over.
+ *   - Record results are not carried: on the clone the records getters answer as after a call that took no records.
+ *   - The clone's launch count starts at 0 and it holds no bound call; pwpp_destroy releases it like any ctx. */
+int pwpp_clone(const pwpp_ctx* src, int device /* < 0: src's device */, pwpp_ctx** out);
+
 /* Re-initialises stream f / all streams to the constructor state (a fresh PatchWorkpp instance).
  * Stream-ordered: enqueued behind the last estimate call, no host synchronization. */
 int pwpp_reset_stream(pwpp_ctx* ctx, int f);

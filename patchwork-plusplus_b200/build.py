@@ -128,6 +128,17 @@ def build_examples(force=False):
     if force or _newer(out12, [src12] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out12, src12])
+    # the device state copies alone, the same way (GPU cases of tests/test_state_copy_backends.py)
+    src13 = os.path.join(REPO, "tests", "gpu_state_copy_probe.cu")
+    out13 = os.path.join(LIB, "libpwpp_state_copy_probe.so")
+    if force or _newer(out13, [src13] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out13, src13])
+    src14 = os.path.join(REPO, "tests", "pwpp_copy_driver.cpp")   # copies of the drop-in class against the real engine (GPU test)
+    out14 = os.path.join(LIB, "pwpp_copy_driver")
+    if force or _newer(out14, [src14, hdr, core]):
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + os.path.join(REPO, "include"), src14, "-o", out14,
+                               "-L" + LIB, "-lpwpp_b200", "-Wl,-rpath,$ORIGIN"])
     return out
 
 

@@ -19,6 +19,7 @@
 #include "pwpp_kernels.cuh"
 #include "pwpp_records.cuh"
 #include "pwpp_getters.cuh"
+#include "pwpp_state_copy.cuh"
 #include "pwpp_tuning.h"
 #include "pwpp_host.hpp"
 
@@ -144,6 +145,7 @@ constexpr int NUM_SIDE = 6;
 struct pwpp_ctx {
   // parameter sets (pwpp_create: one) and the set of every stream; the kernels get the set records by value
   int num_sets = 1;
+  std::vector<pwpp_params> set_params;      // the sets as created (pwpp_clone)
   GeometrySets gs;                          // gs.nbs: the largest bin count of the sets, stride of the per-frame bin arrays
   AlgoParamSets aps;
   bool set_fast[MAX_PARAM_SETS] = {};       // build_geometry: the fp32 binning filter is exact for the set's geometry
@@ -169,6 +171,8 @@ struct pwpp_ctx {
   DevBuf<StreamState> d_states;
   DevBuf<StreamState> d_states_init;  // constructor state of every stream (reset source)
   DevBuf<double> d_hist;
+  DevBuf<int> d_stream_hcap;          // [num_streams] history capacity of every stream's set (device state copies)
+  DevBuf<int> d_claim;                // [num_streams] claim table of pwpp_import_states_device, -1 between calls
 
   // per-call work buffers
   DevBuf<float4> d_in;            // host path only
@@ -969,6 +973,7 @@ static int create_impl(const pwpp_params* sets, int num_sets, const int32_t* str
   ctx->stream_set.assign(num_streams, 0);
   if (stream_set) ctx->stream_set.assign(stream_set, stream_set + num_streams);
   ctx->num_sets = num_sets;
+  ctx->set_params.assign(sets, sets + num_sets);
   ctx->gs.nbs = 0;
   int max_sectors = 0;
   for (int k = 0; k < num_sets; ++k) {
@@ -1021,6 +1026,14 @@ static int create_impl(const pwpp_params* sets, int num_sets, const int32_t* str
   // history samples past a stream's counts are never read by the kernels, but pwpp_export_state copies whole rows: zeroed, a
   // blob holds no bytes of whatever the allocation held before
   CU_TRY_CTX(cudaMemset(ctx->d_hist.p, 0, (size_t) num_streams * 2 * 4 * ctx->hist_stride * sizeof(double)));
+  {
+    std::vector<int> hcap(num_streams);
+    for (int i = 0; i < num_streams; ++i) hcap[i] = ctx->set_hcap[ctx->stream_set[i]];
+    CU_TRY_CTX(ctx->d_stream_hcap.reserve(num_streams));
+    CU_TRY_CTX(cudaMemcpy(ctx->d_stream_hcap.p, hcap.data(), hcap.size() * sizeof(int), cudaMemcpyHostToDevice));
+    CU_TRY_CTX(ctx->d_claim.reserve(num_streams));
+    CU_TRY_CTX(cudaMemset(ctx->d_claim.p, 0xff, (size_t) num_streams * sizeof(int)));
+  }
   CU_TRY_CTX(ctx->d_counts.reserve((size_t) 3 * num_streams));
   CU_TRY_CTX(ctx->d_wq_ctr.reserve(2 * NUM_CLASSES + 2 * ORD_NUM_HEADS));
   CU_TRY_CTX(ctx->d_ox_counts.reserve(OX_NUM_STATS));
@@ -2129,12 +2142,8 @@ int pwpp_copy_history(pwpp_ctx* ctx, int f, int ring, int which, double* dst) {
   return PWPP_OK;
 }
 
-namespace {
-struct StateBlobHeader { uint32_t magic, version; int32_t hcap, state_bytes; };
-constexpr uint32_t STATE_BLOB_MAGIC = 0x50575354u;  // "PWST"
-}  // namespace
 // a stream's blob: header, state, then its eight history rows of its own set's capacity (the layout of a one-set context)
-static size_t blob_size_of_cap(int hcap) { return sizeof(StateBlobHeader) + sizeof(StreamState) + (size_t) 2 * 4 * hcap * sizeof(double); }
+static size_t blob_size_of_cap(int hcap) { return state_blob_bytes(hcap); }
 size_t pwpp_stream_state_blob_size(const pwpp_ctx* ctx, int s) {
   if (!ctx || s < 0 || s >= ctx->num_streams) return 0;
   return blob_size_of_cap(ctx->set_hcap[ctx->stream_set[s]]);
@@ -2173,6 +2182,119 @@ int pwpp_import_state(pwpp_ctx* ctx, int f, const void* blob, size_t bytes) {
   CU_TRY(cudaMemcpy2D(ctx->d_hist.p + (size_t) f * 2 * 4 * ctx->hist_stride, (size_t) ctx->hist_stride * sizeof(double), b + sizeof h + sizeof(StreamState),
                       (size_t) hcap * sizeof(double), (size_t) hcap * sizeof(double), 2 * 4, cudaMemcpyHostToDevice));
   return PWPP_OK;
+}
+
+// The host checks of pwpp_export_states_device / pwpp_import_states_device; *run = false when there is nothing to launch.
+static int check_state_list(const pwpp_ctx* ctx, int n, const int32_t* d_streams, const void* d_blobs, int64_t blob_stride, bool* run) {
+  *run = false;
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (n < 0 || n > 65535) return fail(PWPP_ERR_INVALID_ARG, "n must be in [0, 65535], got " + std::to_string(n));
+  if (n > 0 && (!d_streams || !d_blobs)) return fail(PWPP_ERR_INVALID_ARG, "d_streams and d_blobs must not be NULL when n > 0");
+  const int64_t need = (int64_t) pwpp_state_blob_size(ctx);
+  if (blob_stride < need || blob_stride % 16 != 0)
+    return fail(PWPP_ERR_INVALID_ARG, "blob_stride " + std::to_string(blob_stride) + " must be a multiple of 16 and at least pwpp_state_blob_size = " +
+                                          std::to_string(need));
+  if (reinterpret_cast<uintptr_t>(d_blobs) % 16 != 0) return fail(PWPP_ERR_INVALID_ARG, "d_blobs must be 16-byte aligned");
+  *run = n > 0;
+  return PWPP_OK;
+}
+static StateStore state_store(pwpp_ctx* ctx) {
+  return StateStore{ctx->d_states.p, reinterpret_cast<long long*>(ctx->d_hist.p), ctx->hist_stride, ctx->d_stream_hcap.p, ctx->num_streams};
+}
+
+int pwpp_export_states_device(pwpp_ctx* ctx, int n, const int32_t* d_streams, void* d_blobs, int64_t blob_stride, int32_t* d_status, void* cuda_stream) {
+  bool run = false;
+  int rc = check_state_list(ctx, n, d_streams, d_blobs, blob_stride, &run);
+  if (rc || !run) return rc;
+  rc = bind_device(ctx);
+  if (rc) return rc;
+  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
+  k_state_export<<<n, SC_THREADS, 0, s>>>(d_streams, state_store(ctx), static_cast<unsigned char*>(d_blobs), blob_stride, d_status);
+  ++ctx->launches;
+  CU_TRY(cudaGetLastError());
+  return PWPP_OK;
+}
+
+int pwpp_import_states_device(pwpp_ctx* ctx, int n, const int32_t* d_streams, const void* d_blobs, int64_t blob_stride, int32_t* d_status,
+                              void* cuda_stream) {
+  bool run = false;
+  int rc = check_state_list(ctx, n, d_streams, d_blobs, blob_stride, &run);
+  if (rc || !run) return rc;
+  rc = bind_device(ctx);
+  if (rc) return rc;
+  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
+  k_state_import_claim<<<(n + SC_CLAIM_THREADS - 1) / SC_CLAIM_THREADS, SC_CLAIM_THREADS, 0, s>>>(n, d_streams, ctx->num_streams, ctx->d_claim.p);
+  ++ctx->launches;
+  CU_TRY(cudaGetLastError());
+  k_state_import<<<n, SC_THREADS, 0, s>>>(d_streams, state_store(ctx), static_cast<const unsigned char*>(d_blobs), blob_stride, ctx->d_claim.p, d_status);
+  ++ctx->launches;
+  CU_TRY(cudaGetLastError());
+  return PWPP_OK;
+}
+
+// bytes from src's buffer on device src_dev to dst's on dst_dev, on stream s of dst_dev
+static cudaError_t copy_between(void* dst, int dst_dev, const void* src, int src_dev, size_t bytes, cudaStream_t s) {
+  if (bytes == 0) return cudaSuccess;
+  if (dst_dev == src_dev) return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
+  return cudaMemcpyPeerAsync(dst, dst_dev, src, src_dev, bytes, s);
+}
+
+int pwpp_clone(const pwpp_ctx* src_c, int device, pwpp_ctx** out) {
+  if (!out) return fail(PWPP_ERR_INVALID_ARG, "out is NULL");
+  *out = nullptr;
+  if (!src_c) return fail(PWPP_ERR_INVALID_ARG, "src is NULL");
+  pwpp_ctx* src = const_cast<pwpp_ctx*>(src_c);   // fetching the last call's host description caches it; nothing observable changes
+  if (src->bound.on) return fail(PWPP_ERR_INVALID_ARG, "pwpp_clone: the source holds a bound call; pwpp_unbind_call first");
+  if (device < 0) device = src->device;
+  int rc = bind_device(src);
+  if (rc) return rc;
+  if (src->last_stream) CU_TRY(cudaStreamSynchronize(src->last_stream));
+  CU_TRY(cudaStreamSynchronize(src->stream));
+  const int nf = src->last_nframes;
+  if (nf > 0) {
+    rc = fetch_counts(src);   // the host offsets of a bound call's results (after an unbind) come with the counts
+    if (rc) return rc;
+  }
+  pwpp_ctx* c = nullptr;
+  rc = create_impl(src->set_params.data(), src->num_sets, src->stream_set.data(), device, src->num_streams, 0, &c);
+  if (rc) return rc;
+  auto done = [&](int code) { if (code) pwpp_destroy(c); else *out = c; return code; };
+  const int sd = src->device;
+  cudaStream_t s = c->stream;
+  c->order_mode = src->order_mode;
+#define CU_CLONE(expr) do { const cudaError_t _e = (expr); if (_e != cudaSuccess) return done(fail(PWPP_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e))); } while (0)
+  // the point capacity of src's per-point buffers
+  CU_CLONE(c->d_in.reserve(src->d_in.cap));
+  CU_CLONE(c->d_bin_ids.reserve(src->d_bin_ids.cap));
+  CU_CLONE(c->d_sorted.reserve(src->d_sorted.cap));
+  CU_CLONE(c->d_part.reserve(src->d_part.cap));
+  CU_CLONE(c->d_out_idx.reserve(src->d_out_idx.cap));
+  const size_t ns = (size_t) src->num_streams;
+  CU_CLONE(copy_between(c->d_states.p, device, src->d_states.p, sd, ns * sizeof(StreamState), s));
+  CU_CLONE(copy_between(c->d_hist.p, device, src->d_hist.p, sd, ns * 2 * 4 * src->hist_stride * sizeof(double), s));
+  if (nf > 0) {
+    const long long total = src->last_total;
+    const size_t nb = (size_t) src->gs.nbs;
+    rc = reserve_work(c, nf, total, 0, true, false);
+    if (rc) return done(rc);
+    CU_CLONE(copy_between(c->d_counts.p, device, src->d_counts.p, sd, (size_t) 3 * nf * sizeof(int), s));
+    CU_CLONE(copy_between(c->d_out_idx.p, device, src->d_out_idx.p, sd, (size_t) total * sizeof(int), s));
+    CU_CLONE(copy_between(c->d_in.p, device, src->last_pts, sd, (size_t) total * sizeof(float4), s));
+    CU_CLONE(copy_between(c->d_bin_ids.p, device, src->d_bin_ids.p, sd, (size_t) total * sizeof(unsigned short), s));
+    CU_CLONE(copy_between(c->d_fits.p, device, src->d_fits.p, sd, nf * nb * sizeof(BinFit), s));
+    CU_CLONE(copy_between(c->d_centers.p, device, src->d_centers.p, sd, nf * nb * 3 * sizeof(float), s));
+    CU_CLONE(copy_between(c->d_normals.p, device, src->d_normals.p, sd, nf * nb * 3 * sizeof(float), s));
+    c->last_nframes = nf;
+    c->last_total = total;
+    c->pt_off = src->pt_off;
+    c->frame_set = src->frame_set;
+    c->last_pts = c->d_in.p;
+    c->last_stream = s;
+  }
+  c->last_time_us = src->last_time_us;
+  CU_CLONE(cudaStreamSynchronize(s));
+#undef CU_CLONE
+  return done(PWPP_OK);
 }
 
 int pwpp_device_results(pwpp_ctx* ctx, const int32_t** d_indices, const int32_t** d_num_ground) {

@@ -92,6 +92,9 @@ def load_library():
     lib.pwpp_bound_record_results.restype = i32
     lib.pwpp_bind_getter_results.argtypes = [vp, i32]; lib.pwpp_bind_getter_results.restype = i32
     lib.pwpp_bound_getter_results.argtypes = [vp, C.POINTER(PwppBoundGetters)]; lib.pwpp_bound_getter_results.restype = i32
+    lib.pwpp_export_states_device.argtypes = [vp, i32, vp, vp, i64, vp, vp]; lib.pwpp_export_states_device.restype = i32
+    lib.pwpp_import_states_device.argtypes = [vp, i32, vp, vp, i64, vp, vp]; lib.pwpp_import_states_device.restype = i32
+    lib.pwpp_clone.argtypes = [vp, i32, C.POINTER(vp)]; lib.pwpp_clone.restype = i32
     _lib = lib
     return lib
 
@@ -174,6 +177,7 @@ class Engine:
             _check(self.lib.pwpp_create(C.byref(self.params), device, num_streams, max_points_per_frame, C.byref(h)))
             self.stream_set = [0] * num_streams
         self._h = h
+        self.device = device
         self.num_streams = num_streams
         self.nbins = self.lib.pwpp_num_bins(h)   # with several sets: the largest bin count of the sets
         self._n = []
@@ -732,6 +736,85 @@ class Engine:
 
     def import_state(self, f, blob: bytes):
         _check(self.lib.pwpp_import_state(self._h, f, blob, len(blob)))
+
+    # ---- stream state on the GPU (pwpp_export_states_device / pwpp_import_states_device / pwpp_clone) ----
+    STATE_OK, STATE_SKIPPED, STATE_OUT_OF_RANGE, STATE_BLOB_MISMATCH, STATE_DUPLICATE = 0, 1, 2, 3, 4
+
+    def state_blob_size(self) -> int:
+        """pwpp_state_blob_size: the largest stream blob of the ctx (a row of export_states holds any stream's)."""
+        return int(self.lib.pwpp_state_blob_size(self._h))
+
+    def _state_list(self, streams):
+        """The stream list as a device int32 tensor: a device tensor is used as it is (a graph may rewrite it between replays),
+        anything else is copied to the ctx's device (not capturable)."""
+        import torch
+        if isinstance(streams, torch.Tensor) and streams.is_cuda:
+            if streams.dtype != torch.int32 or streams.dim() != 1 or not streams.is_contiguous():
+                raise PwppError("a device stream list must be a contiguous 1-D int32 tensor")
+            return streams
+        return torch.as_tensor(np.ascontiguousarray(streams, dtype=np.int32).reshape(-1), device=torch.device("cuda", self.device))
+
+    def _torch_stream(self, stream):
+        """`stream`, or for 0 torch's current stream on the ctx's device (its legacy default stream as cudaStreamLegacy), so that
+        the lists and rows torch wrote and the status tensors returned are ordered with torch's own work."""
+        import torch
+        if stream:
+            return stream
+        return torch.cuda.current_stream(self.device).cuda_stream or 1
+
+    @staticmethod
+    def _blob_rows(t, what):
+        import torch
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.uint8 and t.dim() == 2 and t.stride(1) == 1):
+            raise PwppError(f"{what} must be a CUDA uint8 tensor [n, row_bytes] with contiguous rows")
+        return t.stride(0)
+
+    def export_states(self, streams, out=None, stream: int = 0):
+        """The complete state of stream streams[i] into row i of a device uint8 tensor [n, stride] (stride: the state blob size
+        rounded up to 16 bytes, or out's row stride), each row byte for byte export_state's blob. Returns (rows, status int32[n]):
+        STATE_OK, or STATE_SKIPPED (id < 0) / STATE_OUT_OF_RANGE, whose rows are not written. Enqueued on CUDA stream `stream`
+        (0: torch's current stream) with no host synchronisation, so it may be captured into a CUDA graph. The ctx's own calls
+        are ordered by the caller (estimate_host has finished when it returns)."""
+        import torch
+        ids = self._state_list(streams)
+        n = ids.numel()
+        if out is None:
+            out = torch.empty((n, (self.state_blob_size() + 15) // 16 * 16), dtype=torch.uint8, device=ids.device)
+        stride = self._blob_rows(out, "out")
+        if out.shape[0] < n:
+            raise PwppError(f"out holds {out.shape[0]} rows, the list {n}")
+        status = torch.empty(n, dtype=torch.int32, device=ids.device)
+        _check(self.lib.pwpp_export_states_device(self._h, n, ids.data_ptr(), out.data_ptr(), stride, status.data_ptr(),
+                                                  C.c_void_p(self._torch_stream(stream))))
+        return out, status
+
+    def import_states(self, blobs, streams, stream: int = 0):
+        """Row i of the device uint8 tensor `blobs` into stream streams[i], checked on the GPU as import_state checks a blob.
+        Returns the status int32[n]: STATE_OK, STATE_SKIPPED (id < 0: nothing read or written), STATE_OUT_OF_RANGE,
+        STATE_BLOB_MISMATCH (stream untouched) or STATE_DUPLICATE (an earlier entry names the stream). Capturable; `stream` as
+        for export_states. The host getters see the import once that stream has been synchronized."""
+        import torch
+        ids = self._state_list(streams)
+        n = ids.numel()
+        stride = self._blob_rows(blobs, "blobs")
+        if blobs.shape[0] < n:
+            raise PwppError(f"blobs holds {blobs.shape[0]} rows, the list {n}")
+        status = torch.empty(n, dtype=torch.int32, device=ids.device)
+        _check(self.lib.pwpp_import_states_device(self._h, n, ids.data_ptr(), blobs.data_ptr(), stride, status.data_ptr(),
+                                                  C.c_void_p(self._torch_stream(stream))))
+        return status
+
+    def clone(self, device=None):
+        """pwpp_clone: a new Engine on `device` (None: this one's) with this one's parameter sets, stream states and last call's
+        results; both continue identically. Refused while a call is bound."""
+        h = C.c_void_p()
+        _check(self.lib.pwpp_clone(self._h, -1 if device is None else int(device), C.byref(h)))
+        e = Engine.__new__(Engine)
+        e.__dict__.update(self.__dict__)
+        e._h, e.device = h, self.device if device is None else int(device)
+        e.params = list(self.params) if isinstance(self.params, list) else self.params
+        e._n, e._streams, e._rec_dtypes = None if self._n is None else list(self._n), list(self._streams), []
+        return e
 
     def device_index_lists(self):
         """Zero-copy view of the last call's results on the device: (indices, num_ground) as torch int32 CUDA tensors.
