@@ -503,6 +503,50 @@ int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read);
 int pwpp_bind_call_packed(pwpp_ctx* ctx, int nframes, const int32_t* streams, const void* base, const pwpp_point_layout* layout,
                           int64_t capacity /* records at base */, const int64_t* max_n, const int64_t* d_offsets /* device [nframes + 1] */,
                           const int32_t* d_actions /* NULL: all RUN */);
+
+/* A stream table for a bound call: which sensor stream each frame position serves, read on the GPU at every run or replay, so
+ * one bound call (and one captured graph) serves more streams than it has frames, picked per tick by a scheduler on the GPU.
+ *
+ * pwpp_bind_stream_table: enables the table for the bound call, whichever bind made it (plain, actions, rings or packed). From
+ * then on every run or replay reads frame f's stream from d_streams[f], a device int32 array of nframes entries.
+ *   - Runs stay the bind's. The runs are still those of the bound streams (maximal groups of consecutive positions with
+ *     pairwise distinct streams): they fix the launch sequence, the grids and the scratch slots. Bind distinct streams (for
+ *     example 0..F-1) for one run; bind a shape with a repeat (for example [0..63, 0..31]) for two runs, room for a backlog.
+ *     The bound stream values matter only for this shape.
+ *   - Reading. The run's first kernel reads each entry once into a copy the ctx owns (pwpp_bound_call_streams); the later
+ *     kernels read the copy. Frame f's parameter set is stream_set[d_streams[f]], taken on the GPU from a copy of the ctx's
+ *     stream-to-set map made at enable time.
+ *   - Validation (a replay cannot return an error). s < 0 is a hole: the frame is skipped with PWPP_FRAME_SKIPPED, exactly as
+ *     an action SKIP. s >= num_streams: skipped, PWPP_STREAM_OUT_OF_RANGE. Two frames of one run that would run and name the
+ *     same stream: the lowest position runs, the others are skipped with PWPP_STREAM_DUPLICATE; frames skipped by their action
+ *     claim nothing. A skipped frame goes to its scratch slot as an action SKIP does: no real stream is written and a RESET on
+ *     it does not apply.
+ *   - Precedence: the action (SKIP or an invalid action), then the stream (hole, out of range, duplicate), then the ring slot
+ *     or the packed offsets, then the count. A frame rejected by its action or its stream reads no slot, offset or count.
+ *   - Resets. RESET frames of the first run are reset in the table kernel; before every later run a reset launch treats all
+ *     of that run's RESET frames as repeats of an earlier run's stream. So pwpp_launch_count rises, over the same call bound
+ *     without actions, by exactly runs - 1 per run or replay when actions and a stream table are both bound (the same count as
+ *     with actions alone: every later run of a bind already repeats a stream), and a stream table without actions adds nothing.
+ *   - Getter rows (PWPP_GETTER_STATE) follow the stream each frame read: for a frame skipped by its action or as a duplicate,
+ *     its stream's state after the frame's run; for a hole or an out-of-range id the row is not written. Every other result
+ *     (indices, offsets, status, records, xyz, packed results) is indexed by position, as without a table.
+ *   - Host getters. pwpp_copy_bin_results fetches the sets the run used from the device with its first copy after a run; a
+ *     frame rejected with an invalid id reports the set of its bound stream. The fp32 binning filter is used for a run only
+ *     when every set of the ctx allows it (both binning paths are exact: results do not change).
+ *   - Identity. d_streams[f] == streams[f] for every f gives the results of the same bind without a table, bit for bit.
+ *   - Enable-time work. Enabling is host work that synchronizes and must come before the bound call's first run (capture
+ *     included): it grows the state and history buffers by the scratch slots (the longest run) if actions did not already,
+ *     and those must not move under a captured graph. PWPP_ERR_INVALID_ARG for no bound call, NULL d_streams, a second enable
+ *     or an enable after a run; the bound call is then unchanged. pwpp_unbind_call releases the table.
+ *   - Memory: 4 bytes per frame for the copy, 8 bytes per stream for the claim table and the set map.
+ *
+ * pwpp_bound_call_streams: host-only. The ctx's copy of the streams the last run read, device int32[nframes] at a fixed address
+ * while the call stays bound (invalid values included); -1 everywhere before the first run. PWPP_ERR_INVALID_ARG when no call
+ * is bound or it has no stream table. */
+#define PWPP_STREAM_OUT_OF_RANGE 6   /* d_status[f]: d_streams[f] >= num_streams; the frame was skipped */
+#define PWPP_STREAM_DUPLICATE 7      /* d_status[f]: an earlier frame of the same run names the same stream; skipped */
+int pwpp_bind_stream_table(pwpp_ctx* ctx, const int32_t* d_streams /* device int32[nframes] */);
+int pwpp_bound_call_streams(pwpp_ctx* ctx, const int32_t** d_streams_read);
 int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream);
 int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int64_t** d_offsets, const int32_t** d_num_ground,
                             const int32_t** d_status);

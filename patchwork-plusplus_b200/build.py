@@ -134,6 +134,12 @@ def build_examples(force=False):
     if force or _newer(out13, [src13] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out13, src13])
+    # the kernels of bound calls with a stream table, the same way (GPU cases of tests/test_bound_streams_backends.py)
+    src15 = os.path.join(REPO, "tests", "gpu_bound_streams_probe.cu")
+    out15 = os.path.join(LIB, "libpwpp_bound_streams_probe.so")
+    if force or _newer(out15, [src15] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out15, src15])
     src14 = os.path.join(REPO, "tests", "pwpp_copy_driver.cpp")   # copies of the drop-in class against the real engine (GPU test)
     out14 = os.path.join(LIB, "pwpp_copy_driver")
     if force or _newer(out14, [src14, hdr, core]):

@@ -288,8 +288,16 @@ struct pwpp_ctx {
                                                      // on the device at every run when either is enabled
     int packed_rec = 0;                     // packed records (pwpp_bind_packed_records): PWPP_PART_* bits, 0 = off
     DevBuf<unsigned char, false> d_prec_g, d_prec_ng;   // [sum(max_n)][point_step] packed ground / non-ground records
+    const int* d_streams = nullptr;         // the caller's device streams (pwpp_bind_stream_table), NULL: the bound stream table
+    DevBuf<int, false> d_bread;             // [F] with a stream table: the run's copy of the streams
+    DevBuf<int, false> d_bclaim;            // [num_streams] its duplicate claims, -1 between runs
+    DevBuf<int, false> d_bset_of;           // [num_streams] stream_set, for the sets of the streams read on the device
+    DevBuf<int, false> d_bruns;             // [runs + 1] runs, for the duplicate check run by run
+    bool ran = false;                       // a run was enqueued or captured: the state buffers may no longer move
   } bound;
   int scratch_slots = 0;                  // state / history slots after the streams' (pwpp_bind_call_actions), kept after unbind
+  bool sets_on_device = false;            // the last call's sets were picked on the device (a stream table): range_fast asks every
+                                          // set, and fetch_offsets fetches frame_set
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
   struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
@@ -466,14 +474,21 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   ctx->last_nframes = nframes;
   ctx->last_total = total;
   ctx->last_bound = false;
+  ctx->sets_on_device = false;
   ctx->counts_fetched = ctx->idx_fetched = ctx->patches_fetched = false;
   ctx->stage_valid = false;
   return PWPP_OK;
 }
 
 // The fp32 binning filter is used for a launch range only when build_geometry allows it for every set the range names;
-// otherwise the range takes the exact kernel. Both bin exactly, so the bins are the same either way.
+// otherwise the range takes the exact kernel. Both bin exactly, so the bins are the same either way. When the sets are picked on
+// the device (a bound stream table) the host does not know them: every set of the ctx must allow it.
 bool range_fast(const pwpp_ctx* ctx, int f0, int nf) {
+  if (ctx->sets_on_device) {
+    for (int k = 0; k < ctx->num_sets; ++k)
+      if (!ctx->set_fast[k]) return false;
+    return true;
+  }
   for (int f = f0; f < f0 + nf; ++f)
     if (!ctx->set_fast[ctx->frame_set[f]]) return false;
   return true;
@@ -862,7 +877,8 @@ int check_frame(pwpp_ctx* ctx, int f) {
   return PWPP_OK;
 }
 
-// The bound call's point offsets (the device scan of its accepted counts) into the host description of the last call.
+// The bound call's point offsets (the device scan of its accepted counts) into the host description of the last call, and with
+// a stream table the sets its frames ran with.
 int fetch_offsets(pwpp_ctx* ctx) {
   if (!ctx->last_bound || ctx->off_fetched) return PWPP_OK;
   int rc = bind_device(ctx);
@@ -870,6 +886,10 @@ int fetch_offsets(pwpp_ctx* ctx) {
   const int nf = ctx->last_nframes;
   ctx->pt_off.assign(nf + 1, 0);
   CU_TRY(cudaMemcpyAsync(ctx->pt_off.data(), ctx->d_pt_off.p, (size_t) (nf + 1) * sizeof(long long), cudaMemcpyDeviceToHost, ctx->last_stream));
+  if (ctx->sets_on_device) {
+    ctx->frame_set.assign(nf, 0);
+    CU_TRY(cudaMemcpyAsync(ctx->frame_set.data(), ctx->d_pset.p, (size_t) nf * sizeof(int), cudaMemcpyDeviceToHost, ctx->last_stream));
+  }
   CU_TRY(cudaStreamSynchronize(ctx->last_stream));
   ctx->last_total = ctx->pt_off[nf];
   ctx->off_fetched = true;
@@ -1451,6 +1471,7 @@ static void make_bound_last(pwpp_ctx* ctx, cudaStream_t s) {
   ctx->last_stream = s;
   ctx->last_total = 0;
   ctx->last_bound = true;
+  ctx->sets_on_device = b.d_streams != nullptr;
   ctx->off_fetched = ctx->counts_fetched = ctx->idx_fetched = ctx->patches_fetched = false;
   ctx->rec_gathered = ctx->rec_fetched = false;
   ctx->stage_valid = ctx->call_times_valid = false;
@@ -1659,13 +1680,19 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   ctx->last_nframes = nf;
   ctx->runs = b.runs;
   ctx->frame_set = b.frame_set;
+  ctx->sets_on_device = b.d_streams != nullptr;
   ctx->chunk_off = b.cap_chunk_off;
   ctx->pt_off = b.cap_pt_off;
+  ctx->bound.ran = true;
   const BoundActions A{b.d_actions, b.d_bact.p, b.d_bscratch.p, b.d_bdep.p, ctx->d_states_init.p, ctx->d_states.p};
+  const BoundStreams T{b.d_streams, b.d_bread.p, b.d_bclaim.p, b.d_bset_of.p, b.d_bruns.p, (int) b.runs.size() - 1, ctx->num_streams};
   const RecordFrame* recs = b.d_brec.p;   // the record table the unpack and the gather read
   if (b.d_slots) {
     const BoundRings G{b.d_slots, b.d_bslot.p, b.d_bring.p, b.d_brec.p, b.d_brun.p};
-    if (b.d_actions)
+    if (b.d_streams)
+      k_bound_table_rings_streams<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p, ctx->d_stream.p,
+                                                           ctx->d_pset.p, b.d_bstatus.p, A, G, T);
+    else if (b.d_actions)
       k_bound_table_rings_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
                                                            ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, A, G);
     else
@@ -1674,13 +1701,19 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     recs = b.d_brun.p;
   } else if (b.d_offsets) {
     const BoundPacked P{b.d_offsets, b.capacity, b.d_brec.p, b.d_brun.p};
-    if (b.d_actions)
+    if (b.d_streams)
+      k_bound_table_packed_streams<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p, ctx->d_stream.p,
+                                                            ctx->d_pset.p, b.d_bstatus.p, A, P, T);
+    else if (b.d_actions)
       k_bound_table_packed_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
                                                             ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, A, P);
     else
       k_bound_table_packed<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
                                                     ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, P);
     recs = b.d_brun.p;
+  } else if (b.d_streams) {
+    k_bound_table_streams<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, b.d_bmax.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p, ctx->d_stream.p,
+                                                   ctx->d_pset.p, b.d_bstatus.p, A, T);
   } else if (b.d_actions) {
     k_bound_table_actions<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
                                                    ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, A);
@@ -1695,8 +1728,11 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   }
   CU_TRY(cudaGetLastError());
   for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
-    if (b.d_actions && b.reset_run[r]) {   // the RESET frames whose stream ran in an earlier run
-      k_bound_reset<<<1, BR_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bact.p, b.d_bdep.p, b.d_bstream.p, ctx->d_states_init.p, ctx->d_states.p);
+    // the RESET frames whose stream ran in an earlier run; with a stream table the host cannot know which, so every RESET frame
+    // of every later run (its dep is 1) is reset right before its run, from the streams the run read
+    if (b.d_actions && (b.d_streams ? r > 0 : b.reset_run[r])) {
+      k_bound_reset<<<1, BR_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bact.p, b.d_bdep.p, b.d_streams ? b.d_bread.p : b.d_bstream.p,
+                                             ctx->d_states_init.p, ctx->d_states.p);
       ++ctx->launches;
       CU_TRY(cudaGetLastError());
     }
@@ -1704,7 +1740,11 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     if (rc) return rc;
     if (b.getters & PWPP_GETTER_STATE) {   // before a later run moves the run's streams
       const int len = b.runs[r + 1] - b.runs[r];
-      k_bound_states<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bstream.p, ctx->d_states.p, b.d_bstates.p);
+      if (b.d_streams)
+        k_bound_states_streams<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bread.p, ctx->num_streams,
+                                                                                          ctx->d_states.p, b.d_bstates.p);
+      else
+        k_bound_states<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bstream.p, ctx->d_states.p, b.d_bstates.p);
       ++ctx->launches;
       CU_TRY(cudaGetLastError());
     }
@@ -1764,6 +1804,76 @@ int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read) {
   if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call_rings)");
   if (!ctx->bound.d_slots) return fail(PWPP_ERR_INVALID_ARG, "the bound call has no rings (pwpp_bind_call_rings)");
   if (d_slots_read) *d_slots_read = ctx->bound.d_bslot.p;
+  return PWPP_OK;
+}
+
+// With a stream table every frame of run r gets scratch slot num_streams + (f - runs[r]) as with actions, and dep[f] = (r > 0):
+// the table kernel resets the RESET frames of run 0, k_bound_reset those of every later run (the host no longer knows which
+// streams repeat). The tables are built in buffers of their own and moved into the bound call only when all of them exist.
+int pwpp_bind_stream_table(pwpp_ctx* ctx, const int32_t* d_streams) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  pwpp_ctx::Bound& b = ctx->bound;
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (!d_streams) return fail(PWPP_ERR_INVALID_ARG, "d_streams is NULL");
+  if (b.d_streams) return fail(PWPP_ERR_INVALID_ARG, "a stream table is already enabled for the bound call");
+  if (b.ran)
+    return fail(PWPP_ERR_INVALID_ARG, "the bound call has run or been captured: enable its stream table before its first run (the state buffers may grow)");
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const int nf = b.nf, nruns = (int) b.runs.size() - 1, ns = ctx->num_streams;
+  std::vector<int> scratch(nf), dep(nf);
+  int slots = 0;   // the longest run
+  for (int r = 0; r < nruns; ++r) {
+    slots = std::max(slots, b.runs[r + 1] - b.runs[r]);
+    for (int f = b.runs[r]; f < b.runs[r + 1]; ++f) {
+      scratch[f] = ns + (f - b.runs[r]);
+      dep[f] = r > 0;
+    }
+  }
+  // the state buffers may move: whatever the ctx enqueued before has finished with them
+  if (ctx->last_stream) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  CU_TRY(cudaStreamSynchronize(ctx->stream));
+  if (slots > ctx->scratch_slots) {
+    const size_t n = (size_t) ns + slots;
+    CU_TRY(ctx->d_states.grow_keep(n));
+    CU_TRY(ctx->d_hist.grow_keep(n * 2 * 4 * ctx->hist_stride));
+    ctx->scratch_slots = slots;
+  }
+  if (!b.d_actions) {   // (with actions the bind filled them) a scratch slot starts as a constructor state, as in bind_call_impl
+    StreamState s0;
+    CU_TRY(cudaMemcpy(&s0, ctx->d_states_init.p, sizeof(StreamState), cudaMemcpyDeviceToHost));
+    const std::vector<StreamState> fill(slots, s0);
+    CU_TRY(cudaMemcpy(ctx->d_states.p + ns, fill.data(), (size_t) slots * sizeof(StreamState), cudaMemcpyHostToDevice));
+  }
+  DevBuf<int, false> read, claim, set_of, runs, sc, dp;
+  CU_TRY(read.reserve(nf));
+  CU_TRY(claim.reserve(ns));
+  CU_TRY(set_of.reserve(ns));
+  CU_TRY(runs.reserve(nruns + 1));
+  CU_TRY(sc.reserve(nf));
+  CU_TRY(dp.reserve(nf));
+  CU_TRY(cudaMemset(read.p, 0xff, (size_t) nf * sizeof(int)));   // -1: no run yet
+  CU_TRY(cudaMemset(claim.p, 0xff, (size_t) ns * sizeof(int)));
+  CU_TRY(cudaMemcpy(set_of.p, ctx->stream_set.data(), (size_t) ns * sizeof(int), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(runs.p, b.runs.data(), (size_t) (nruns + 1) * sizeof(int), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(sc.p, scratch.data(), (size_t) nf * sizeof(int), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(dp.p, dep.data(), (size_t) nf * sizeof(int), cudaMemcpyHostToDevice));
+  CU_TRY(cudaDeviceSynchronize());
+  b.d_bread = std::move(read);
+  b.d_bclaim = std::move(claim);
+  b.d_bset_of = std::move(set_of);
+  b.d_bruns = std::move(runs);
+  b.d_bscratch = std::move(sc);
+  if (b.d_actions) b.d_bdep = std::move(dp);
+  b.d_streams = d_streams;
+  return PWPP_OK;
+}
+
+int pwpp_bound_call_streams(pwpp_ctx* ctx, const int32_t** d_streams_read) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (!ctx->bound.d_streams) return fail(PWPP_ERR_INVALID_ARG, "the bound call has no stream table (pwpp_bind_stream_table)");
+  if (d_streams_read) *d_streams_read = ctx->bound.d_bread.p;
   return PWPP_OK;
 }
 
@@ -2373,6 +2483,7 @@ int pwpp_bind_host_to_device(int device) {
 int pwpp_copy_bin_results(pwpp_ctx* ctx, int f, pwpp_bin_result* dst) {
   int rc = check_frame(ctx, f);
   if (rc) return rc;
+  if (ctx->sets_on_device && (rc = fetch_offsets(ctx))) return rc;   // the sets the bound call's frames ran with
   rc = bind_device(ctx);
   if (rc) return rc;
   CU_TRY(cudaStreamSynchronize(ctx->last_stream));

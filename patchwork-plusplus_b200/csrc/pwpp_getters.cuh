@@ -121,11 +121,7 @@ inline long long xyz_parts_grid_x(const long long* cap_off, int nf) {
 // frames left it.
 constexpr int BS_THREADS = 128;
 
-__global__ void __launch_bounds__(BS_THREADS) k_bound_states(int f0, int f1, const int* __restrict__ b_stream, const StreamState* __restrict__ states,
-                                                             pwpp_state* __restrict__ out) {
-  const int f = f0 + (int) (blockIdx.x * BS_THREADS + threadIdx.x);
-  if (f >= f1) return;
-  const StreamState& s = states[b_stream[f]];
+__device__ __forceinline__ void bound_state_row(const StreamState& s, pwpp_state* __restrict__ out) {
   pwpp_state r;
   r.sensor_height = s.sensor_height;
 #pragma unroll
@@ -135,7 +131,25 @@ __global__ void __launch_bounds__(BS_THREADS) k_bound_states(int f0, int f1, con
     r.n_elevation[i] = s.n_elev[i];
     r.n_flatness[i] = s.n_flat[i];
   }
-  out[f] = r;
+  *out = r;
+}
+
+__global__ void __launch_bounds__(BS_THREADS) k_bound_states(int f0, int f1, const int* __restrict__ b_stream, const StreamState* __restrict__ states,
+                                                             pwpp_state* __restrict__ out) {
+  const int f = f0 + (int) (blockIdx.x * BS_THREADS + threadIdx.x);
+  if (f >= f1) return;
+  bound_state_row(states[b_stream[f]], out + f);
+}
+
+// The same with a stream table (pwpp_bind_stream_table): the stream is the one frame f read (the run's copy, read). A frame
+// skipped by its action or as a duplicate still names a stream: its row is that stream's state after the run (a duplicate's
+// stream was run by the frame that won it). A hole or an out-of-range id leaves its row as it was.
+__global__ void __launch_bounds__(BS_THREADS) k_bound_states_streams(int f0, int f1, const int* __restrict__ read, int num_streams,
+                                                                     const StreamState* __restrict__ states, pwpp_state* __restrict__ out) {
+  const int f = f0 + (int) (blockIdx.x * BS_THREADS + threadIdx.x);
+  if (f >= f1) return;
+  const int s = read[f];
+  if (s >= 0 && s < num_streams) bound_state_row(states[s], out + f);
 }
 
 }  // namespace pwpp

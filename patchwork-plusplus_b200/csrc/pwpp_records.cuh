@@ -161,6 +161,11 @@ inline RecordFrame record_frame(const pwpp_point_layout& L, const void* src) {
 // 0 <= lo <= hi <= capacity make an empty frame with status PWPP_OFFSETS_OUT_OF_RANGE, a count hi - lo above max_n[f] one with
 // PWPP_COUNT_OUT_OF_RANGE, and an accepted frame's entry brun[f] is brec[f] with src = base + lo * step. Every other frame keeps
 // src = base with n = 0. A skipped frame reads neither offset.
+//
+// With a stream table (pwpp_bind_stream_table), k_bound_table_streams / _rings_streams / _packed_streams take every frame's
+// stream from the caller's device array instead of the bound table: read once into the ctx's copy (bt_stream_verdicts), the
+// set from the device map set_of, holes, out-of-range ids and duplicates inside a run skipped to the scratch slot as an action
+// SKIP is. They always take the actions form (A.actions may be NULL: every frame RUN).
 constexpr int BT_THREADS = 1024;
 
 // The CTA-wide scan of the one-CTA table kernels (bound_table_body, k_bound_xyz_offsets): each of the BT_THREADS threads (lane,
@@ -258,21 +263,70 @@ __device__ __forceinline__ long long bt_packed_count(const BoundPacked& P, int f
   return bt_offsets_ok(lo, hi, P.capacity) ? hi - lo : -1;
 }
 
-template <bool Actions, bool Rings = false, bool Packed = false>
+// the stream table of a bound call (pwpp_bind_stream_table)
+struct BoundStreams {
+  const int* streams;            // the caller's device streams [nf]
+  int* read;                     // the ctx's copy [nf]: what every frame read, invalid values included
+  int* claim;                    // [num_streams] duplicate claims, -1 between runs
+  const int* set_of;             // [num_streams] parameter set of every stream
+  const int* runs;               // [nruns + 1] the bound runs
+  int nruns, num_streams;
+};
+
+// With a stream table, before the count pass: every frame's action (NULL actions: RUN) and stream, read once and copied, and a
+// first verdict in status[f] that the later passes of the same thread read back: the action's skip status, then
+// PWPP_FRAME_SKIPPED for a hole (s < 0), PWPP_STREAM_OUT_OF_RANGE, or, run by run, PWPP_STREAM_DUPLICATE for a frame that would
+// run but whose stream an earlier frame of the run claimed. A claim is an atomicMax of INT_MAX - f on claim[s]: the lowest
+// position wins, and the -1 of an unclaimed entry is below every key. The claims are put back to -1 before the next run.
+// A frame rejected by its stream gets PWPP_FRAME_SKIP in the action copy, so that k_bound_reset leaves its stream alone.
+__device__ __forceinline__ void bt_stream_verdicts(int f0, int f1, const BoundActions& A, const BoundStreams& T, int* __restrict__ status) {
+  for (int f = f0; f < f1; ++f) {
+    const int a = A.actions ? A.actions[f] : PWPP_FRAME_RUN;
+    const int s = T.streams[f];
+    T.read[f] = s;
+    int v = 0;
+    if (!bt_runs(a)) v = a == PWPP_FRAME_SKIP ? PWPP_FRAME_SKIPPED : PWPP_ACTION_INVALID;
+    else if (s < 0) v = PWPP_FRAME_SKIPPED;
+    else if (s >= T.num_streams) v = PWPP_STREAM_OUT_OF_RANGE;
+    if (A.act) A.act[f] = (v != 0 && bt_runs(a)) ? PWPP_FRAME_SKIP : a;
+    status[f] = v;
+  }
+  for (int r = 0; r < T.nruns; ++r) {   // every thread takes part in every run's barriers; its slice may span several runs
+    const int r0 = max(f0, T.runs[r]), r1 = min(f1, T.runs[r + 1]);
+    for (int f = r0; f < r1; ++f)
+      if (status[f] == 0) atomicMax(&T.claim[T.read[f]], 0x7fffffff - f);
+    __syncthreads();
+    for (int f = r0; f < r1; ++f) {
+      if (status[f] != 0) continue;
+      if (*(volatile const int*) &T.claim[T.read[f]] != 0x7fffffff - f) {   // volatile: the claims changed since any earlier load
+        status[f] = PWPP_STREAM_DUPLICATE;
+        if (A.act) A.act[f] = PWPP_FRAME_SKIP;
+      }
+    }
+    __syncthreads();
+    for (int f = r0; f < r1; ++f)
+      if (status[f] == 0) T.claim[T.read[f]] = -1;   // the winner, the one frame of the run left on its stream
+    __syncthreads();
+  }
+}
+
+template <bool Actions, bool Rings = false, bool Packed = false, bool Streams = false>
 __device__ __forceinline__ void bound_table_body(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
                                                  const int* __restrict__ b_stream, const int* __restrict__ b_pset, long long* __restrict__ pt_off,
                                                  int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
                                                  int* __restrict__ status, const BoundActions& A, long long* s_pts, int* s_chk,
-                                                 const BoundRings& G = BoundRings{}, const BoundPacked& P = BoundPacked{}) {
+                                                 const BoundRings& G = BoundRings{}, const BoundPacked& P = BoundPacked{},
+                                                 const BoundStreams& T = BoundStreams{}) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int per = (nf + BT_THREADS - 1) / BT_THREADS;
   const int f0 = tid * per < nf ? tid * per : nf;
   const int f1 = f0 + per < nf ? f0 + per : nf;
   long long own_pts = 0;
   int own_chk = 0;
+  if (Streams) bt_stream_verdicts(f0, f1, A, T, status);
   for (int f = f0; f < f1; ++f) {
     long long n = 0;
-    if (bt_runs(bt_action<Actions>(A, f))) {
+    if (Streams ? status[f] == 0 : bt_runs(bt_action<Actions>(A, f))) {
       const long long c = Packed ? bt_packed_count(P, f) : bt_count<Rings>(counts, G, f);
       n = (c >= 0 && c <= max_n[f]) ? c : 0;
     } else if (Rings) {
@@ -285,7 +339,23 @@ __device__ __forceinline__ void bound_table_body(int nf, const long long* __rest
   int q;
   bt_scan_slices(lane, warp, own_pts, own_chk, p, q, s_pts, s_chk);
   for (int f = f0; f < f1; ++f) {
-    if (Actions) {
+    int sf = 0, ps = 0;   // with a stream table: the frame's stream and set
+    if (Streams) {
+      sf = T.read[f];   // this thread's own copies from the first pass
+      const int v = status[f];
+      if (v != 0) {
+        pt_off[f] = p;
+        chunk_off[f] = q;
+        stream[f] = A.scratch[f];
+        pset[f] = sf >= 0 && sf < T.num_streams ? T.set_of[sf] : b_pset[f];
+        if (Rings) G.brun[f] = G.brec[f];
+        if (Packed) P.brun[f] = P.brec[f];
+        continue;
+      }
+      ps = T.set_of[sf];
+      if (A.act && A.act[f] == PWPP_FRAME_RESET && !A.dep[f]) A.states[sf] = A.init[sf];
+    }
+    if (Actions && !Streams) {
       const int a = A.act[f];   // this thread's own copy from the first pass
       if (!bt_runs(a)) {
         pt_off[f] = p;
@@ -332,8 +402,8 @@ __device__ __forceinline__ void bound_table_body(int nf, const long long* __rest
     pt_off[f] = p;
     chunk_off[f] = q;
     status[f] = ok ? 0 : bad;
-    stream[f] = b_stream[f];
-    pset[f] = b_pset[f];
+    stream[f] = Streams ? sf : b_stream[f];
+    pset[f] = Streams ? ps : b_pset[f];
     p += n;
     q += (int) ((n + CHUNK_PTS - 1) / CHUNK_PTS);
   }
@@ -395,10 +465,43 @@ __global__ void __launch_bounds__(BT_THREADS) k_bound_table_packed_actions(int n
   bound_table_body<true, false, true>(nf, nullptr, max_n, b_stream, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk, BoundRings{}, P);
 }
 
+// The three sources with a stream table (pwpp_bind_stream_table), with or without actions (A.actions NULL: every frame RUN,
+// A.act NULL: no copy, no reset).
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table_streams(int nf, const long long* __restrict__ counts, const long long* __restrict__ max_n,
+                                                                    const int* __restrict__ b_pset, long long* __restrict__ pt_off,
+                                                                    int* __restrict__ chunk_off, int* __restrict__ stream, int* __restrict__ pset,
+                                                                    int* __restrict__ status, const BoundActions A, const BoundStreams T) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<true, false, false, true>(nf, counts, max_n, nullptr, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk,
+                                             BoundRings{}, BoundPacked{}, T);
+}
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table_rings_streams(int nf, const long long* __restrict__ max_n, const int* __restrict__ b_pset,
+                                                                          long long* __restrict__ pt_off, int* __restrict__ chunk_off,
+                                                                          int* __restrict__ stream, int* __restrict__ pset, int* __restrict__ status,
+                                                                          const BoundActions A, const BoundRings G, const BoundStreams T) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<true, true, false, true>(nf, nullptr, max_n, nullptr, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk, G,
+                                            BoundPacked{}, T);
+}
+
+__global__ void __launch_bounds__(BT_THREADS) k_bound_table_packed_streams(int nf, const long long* __restrict__ max_n, const int* __restrict__ b_pset,
+                                                                           long long* __restrict__ pt_off, int* __restrict__ chunk_off,
+                                                                           int* __restrict__ stream, int* __restrict__ pset, int* __restrict__ status,
+                                                                           const BoundActions A, const BoundPacked P, const BoundStreams T) {
+  __shared__ long long s_pts[BT_THREADS / 32];
+  __shared__ int s_chk[BT_THREADS / 32];
+  bound_table_body<true, false, true, true>(nf, nullptr, max_n, nullptr, b_pset, pt_off, chunk_off, stream, pset, status, A, s_pts, s_chk,
+                                            BoundRings{}, P, T);
+}
+
 // k_bound_reset: one CTA before run [f0, f1) of a bound call with actions, launched only for runs that hold a frame whose stream
 // has a frame in an earlier run. Every such frame whose action (the run's copy, act) is PWPP_FRAME_RESET restores its stream's
 // constructor state: the StreamState only, as pwpp_reset_stream (the history sizes live in it). The run's streams are
-// pairwise distinct, so no two threads write one state.
+// pairwise distinct, so no two threads write one state. With a stream table it runs before every run after the first, over the
+// run's copy of the streams (every dep is 1 there; a frame its stream rejected has SKIP in the action copy).
 constexpr int BR_THREADS = 128;
 
 __global__ void __launch_bounds__(BR_THREADS) k_bound_reset(int f0, int f1, const int* __restrict__ act, const int* __restrict__ dep,

@@ -80,6 +80,8 @@ def load_library():
     lib.pwpp_bind_call_rings.argtypes = [vp, i32, vp, C.POINTER(PwppScanRing), vp, vp, vp, vp]; lib.pwpp_bind_call_rings.restype = i32
     lib.pwpp_bound_call_slots.argtypes = [vp, C.POINTER(vp)]; lib.pwpp_bound_call_slots.restype = i32
     lib.pwpp_bind_call_packed.argtypes = [vp, i32, vp, vp, C.POINTER(PwppPointLayout), i64, vp, vp, vp]; lib.pwpp_bind_call_packed.restype = i32
+    lib.pwpp_bind_stream_table.argtypes = [vp, vp]; lib.pwpp_bind_stream_table.restype = i32
+    lib.pwpp_bound_call_streams.argtypes = [vp, C.POINTER(vp)]; lib.pwpp_bound_call_streams.restype = i32
     lib.pwpp_bind_packed_xyz.argtypes = [vp, i32]; lib.pwpp_bind_packed_xyz.restype = i32
     lib.pwpp_bound_packed_xyz.argtypes = [vp] + [C.POINTER(vp)] * 4; lib.pwpp_bound_packed_xyz.restype = i32
     lib.pwpp_bind_packed_records.argtypes = [vp, i32]; lib.pwpp_bind_packed_records.restype = i32
@@ -112,6 +114,7 @@ class PwppError(RuntimeError):
 FRAME_RUN, FRAME_SKIP, FRAME_RESET = 0, 1, 2
 FRAME_SKIPPED, ACTION_INVALID = 2, 3
 SLOT_OUT_OF_RANGE = 4   # status of a ring-bound frame whose slot is outside its ring (PWPP_SLOT_OUT_OF_RANGE)
+STREAM_OUT_OF_RANGE, STREAM_DUPLICATE = 6, 7   # statuses of a stream table's rejected frames (PWPP_STREAM_*)
 
 
 # sensor_msgs/PointField datatype codes (PWPP_FIELD_* of include/pwpp.h) of the numpy scalar types
@@ -186,6 +189,7 @@ class Engine:
         self._bound = None      # (frames, counts, streams, sum of max_n) of the bound call
         self._bound_actions = None   # its actions tensor (bind_call(actions=...)), kept alive while bound
         self._bound_rings = None     # its ring tensors and slots (bind_call_rings), kept alive while bound
+        self._bound_streams = None   # its stream table (bind_stream_table), kept alive while bound
 
     def close(self):
         if getattr(self, "_h", None):
@@ -486,6 +490,34 @@ class Engine:
                 self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<i4", "data": (ptr, False), "version": 3, "strides": None}
         return torch.as_tensor(_View(a.value, nf), device="cuda")
 
+    def bind_stream_table(self, streams):
+        """Reads every frame's stream of the bound call from `streams`, a contiguous int32 CUDA tensor of nframes entries, at every
+        run or replay (pwpp_bind_stream_table): -1 leaves the frame out, an id >= num_streams or a second frame of one run on the
+        same stream is skipped with STREAM_OUT_OF_RANGE / STREAM_DUPLICATE. The runs stay those of the bound streams. Call it
+        before the bound call's first run; the tensor is kept alive while bound and its contents may change between runs."""
+        import torch
+        if self._bound is None:
+            raise PwppError("no call is bound")
+        nf = len(self._bound[2])
+        if not (isinstance(streams, torch.Tensor) and streams.is_cuda and streams.dtype == torch.int32 and streams.is_contiguous()
+                and streams.numel() == nf):
+            raise PwppError(f"streams must be a contiguous int32 CUDA tensor of {nf} entries")
+        _check(self.lib.pwpp_bind_stream_table(self._h, C.c_void_p(streams.data_ptr())))
+        self._bound_streams = streams
+
+    def bound_call_streams(self):
+        """Torch view (int32 [nframes]) of the streams the last run read (pwpp_bound_call_streams): the run's own copy, invalid ids
+        included, -1 before the first run. Fixed address while the call is bound."""
+        import torch
+        a = C.c_void_p()
+        _check(self.lib.pwpp_bound_call_streams(self._h, C.byref(a)))
+        nf = len(self._bound[2])
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr, n):
+                self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<i4", "data": (ptr, False), "version": 3, "strides": None}
+        return torch.as_tensor(_View(a.value, nf), device="cuda")
+
     def run_bound_call(self, stream: int = 0):
         """Enqueues the bound call on CUDA stream `stream` (0: the ctx's own stream; inside torch.cuda.graph pass
         torch.cuda.current_stream().cuda_stream). No host synchronisation: it may be captured and replayed."""
@@ -589,16 +621,25 @@ class Engine:
                 "n_flatness": view(s and s + PwppState.n_flatness.offset, (nf, 4), "<i4", (st, 4))}
 
     def unbind_call(self):
+        if self._bound_streams is not None and self._streams is getattr(self, "_table_streams", None):
+            # the last call keeps its host getters after the unbind: name the streams its frames read (an invalid id: the bound
+            # stream, whose set the frame ran with), so bin_results sizes the records of each frame's set without the table
+            self.synchronize()
+            read = self.bound_call_streams().cpu().tolist()
+            self._streams = [s if 0 <= s < self.num_streams else b for s, b in zip(read, self._bound[2])]
+        self._table_streams = None
         _check(self.lib.pwpp_unbind_call(self._h))
         self._bound = None
         self._bound_actions = None
         self._bound_rings = None
+        self._bound_streams = None
 
     def _use_bound(self):
         """The host getters now serve the bound call: its frame sizes are fetched from the device when first needed."""
         self._n = None
         self._streams = list(self._bound[2])
         self._rec_dtypes = []
+        self._table_streams = self._streams if self._bound_streams is not None else None   # bin_results: sets read on the device
 
     def _sizes(self):
         """Point count of every frame of the last call (after a bound call: from its device offsets, one device->host copy)."""
@@ -704,6 +745,14 @@ class Engine:
 
     def bin_results(self, f=0):
         """Patch records of frame f of the last call: the bins of the frame's parameter set."""
+        if self._streams is getattr(self, "_table_streams", None):
+            # a stream table: the C-ABI writes the bins of the set the frame ran with; the stream it read names that set (an
+            # invalid id: its bound stream's)
+            arr = (PwppBinResult * self.nbins)()
+            _check(self.lib.pwpp_copy_bin_results(self._h, f, C.byref(arr)))
+            s = int(self.bound_call_streams()[f])
+            nb = self.stream_num_bins(s if 0 <= s < self.num_streams else self._streams[f])
+            return (PwppBinResult * nb).from_buffer(arr)
         nb = self.stream_num_bins(self._streams[f]) if 0 <= f < len(self._streams) else self.nbins   # (a bad f: the C-ABI reports it)
         arr = (PwppBinResult * nb)()
         _check(self.lib.pwpp_copy_bin_results(self._h, f, C.byref(arr)))
