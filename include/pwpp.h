@@ -264,8 +264,9 @@ int pwpp_copy_nonground_records(pwpp_ctx* ctx, int f, void* dst);    /* num_nong
 
 /* ---- bound calls: frame sizes read on the GPU, capturable into the caller's CUDA graph --------------------------------------
  * A GPU pipeline often knows a frame's size only on the device (a compaction kernel wrote it, or a static-shape pipeline pads
- * every frame to a capacity and carries the count as a device tensor). A ctx holds at most one BOUND call: its frames, their
- * capacities, the device array of their counts and the stream table, fixed once by pwpp_bind_call. Running it needs only a
+ * every frame to a capacity and carries the count as a device tensor). A BOUND call holds its frames, their capacities, the
+ * device array of their counts and the stream table, fixed once by pwpp_bind_call. A ctx holds up to PWPP_MAX_BOUND_CALLS of
+ * them; every entry point below acts on the selected one (pwpp_select_bound_call, "Several bound calls"). Running it needs only a
  * CUDA stream, performs no host synchronisation, and may be captured into the caller's CUDA graph; every run or replay reads
  * the current counts and frame contents.
  *
@@ -614,6 +615,51 @@ int pwpp_bound_getter_results(pwpp_ctx* ctx, pwpp_bound_getters* out);
 /* Releases the bound call, its record results and its getter results (PWPP_ERR_INVALID_ARG when none is bound). Its index results stay readable
  * until the next call. */
 int pwpp_unbind_call(pwpp_ctx* ctx);
+
+/* ---- several bound calls: one captured graph per batch shape over the same sensor streams ----------------------------------
+ * A pipeline that replays CUDA graphs captures one graph per batch shape and picks one per step (a bucket ladder of 1, 4, 16
+ * and 64 frames), or keeps a ring-bound live graph beside a packed graph of logged scans. A ctx holds bound calls 0 ..
+ * PWPP_MAX_BOUND_CALLS - 1, each with its own shape (frames, capacities, bind kind, runs), over the ctx's one set of streams.
+ *
+ * pwpp_select_bound_call: selects bound call k. Host-only: no synchronisation and no launch. k outside
+ * [0, PWPP_MAX_BOUND_CALLS) returns PWPP_ERR_INVALID_ARG and the selection is unchanged. Call 0 is selected when the ctx is
+ * created, so a caller that never selects has the one bound call described above.
+ * pwpp_selected_bound_call: the selected call (PWPP_ERR_INVALID_ARG for a NULL ctx).
+ *
+ * Every bind (pwpp_bind_call, _actions, _rings, _packed), pwpp_bind_stream_table, pwpp_bind_record_results,
+ * pwpp_bind_getter_results, pwpp_bind_packed_xyz, pwpp_bind_packed_records, pwpp_run_bound_call, every pwpp_bound_* getter and
+ * pwpp_unbind_call act on the selected call, with the semantics above. A bind on a selected call that is already bound returns
+ * PWPP_ERR_INVALID_ARG ("already bound"). A graph captured from pwpp_run_bound_call holds the call selected at capture: a
+ * later selection has no effect on it.
+ *
+ * Rules:
+ *   - Shared. All bound calls share the stream states and histories, the parameter sets, the output order, the scratch state
+ *     slots (as many as the longest run of any call) and the work buffers. So the caller orders runs and replays of different
+ *     calls as it orders direct calls: on one CUDA stream, or with its own events. Replays of two bound calls of one ctx at the
+ *     same time are not supported.
+ *   - Per call. Each call has its own device tables and status array, its copies of the actions, ring slots and streams, the
+ *     claim table of its stream table, and its record, getter (xyz and state), packed-xyz and packed-record buffers. They hold
+ *     that call's last run until its next run: runs of other calls and direct calls never write them. The index results
+ *     (d_indices, d_offsets, d_num_ground of pwpp_bound_call_results) and the patch rows of pwpp_bound_getter_results live in
+ *     the work buffers: they hold the last run of any call (or the last direct call).
+ *   - Growth. A bind may need larger work buffers (sum(max_n) points, nframes frames; under PWPP_ORDER_REFERENCE_EXACT also the
+ *     fix-up's scratch) and a bind with actions or a stream-table enable more scratch slots. Before any bound call has run or
+ *     been captured they grow as needed. Afterwards captured graphs hold them, so such a bind or enable returns
+ *     PWPP_ERR_CAPACITY before anything changes; the message names the points and frames or the scratch slots it needs. To
+ *     avoid it, bind every call, widest shape first (each buffer then grows once), and enable its tables before the first run
+ *     or capture. Creating the
+ *     ctx with a large enough max_points_per_frame pre-sizes the work buffers, not the scratch slots: only binds make those.
+ *   - Freeze. The freeze of the work buffers holds while any call is bound: a direct call that would grow a buffer returns
+ *     PWPP_ERR_CAPACITY, pwpp_set_output_order and pwpp_clone return PWPP_ERR_INVALID_ARG. pwpp_unbind_call releases only the
+ *     selected call; it moves no shared buffer, so the graphs of the other calls stay valid.
+ *   - Host getters follow the last call: the bound call whose pwpp_run_bound_call or pwpp_bound_call_results came last, not
+ *     the selected one. Unbinding it leaves its index results readable until the next call. A bind ends the last call's
+ *     results, as with one bound call.
+ *   - pwpp_launch_count rises per run exactly as for the same call bound alone in a fresh ctx.
+ *   - Memory: each bound call's own tables and result buffers, as described for its bind; nothing else per call. */
+#define PWPP_MAX_BOUND_CALLS 32
+int pwpp_select_bound_call(pwpp_ctx* ctx, int k);
+int pwpp_selected_bound_call(const pwpp_ctx* ctx);
 
 /* cudaDeviceSynchronize() on the ctx's device: what a binding calls before handing device memory produced on an unknown
  * stream to pwpp_estimate_device (and what makes its results visible to every stream afterwards). */

@@ -244,10 +244,11 @@ struct pwpp_ctx {
   bool rec_gathered = false, rec_fetched = false;
   double last_time_us = 0.0;
   cudaStream_t last_stream = nullptr;
-  bool last_bound = false, off_fetched = false;   // the last call is the bound call; its point offsets were fetched (fetch_offsets)
+  int last_call = -1;             // the bound call that is the last call (make_bound_last), -1: a direct call
+  bool off_fetched = false;       // the last call's point offsets were fetched (fetch_offsets)
 
-  // the bound call (pwpp_bind_call): what its runs re-establish and launch, and the device buffers it owns (released with it).
-  // The work buffers are frozen while it is bound.
+  // a bound call (pwpp_bind_call): what its runs re-establish and launch, and the device buffers it owns (released with it).
+  // The work buffers are frozen while any call is bound.
   struct Bound {
     bool on = false;
     int nf = 0, has_intensity = 0;
@@ -294,8 +295,12 @@ struct pwpp_ctx {
     DevBuf<int, false> d_bset_of;           // [num_streams] stream_set, for the sets of the streams read on the device
     DevBuf<int, false> d_bruns;             // [runs + 1] runs, for the duplicate check run by run
     bool ran = false;                       // a run was enqueued or captured: the state buffers may no longer move
-  } bound;
-  int scratch_slots = 0;                  // state / history slots after the streams' (pwpp_bind_call_actions), kept after unbind
+  };
+  // Bound calls 0 .. PWPP_MAX_BOUND_CALLS - 1. They share the stream states, the scratch slots and the work buffers, so a bind
+  // may grow those only while none of them has run (check_growth).
+  Bound bound[PWPP_MAX_BOUND_CALLS];
+  int sel = 0;                            // the call the bind, run, result and unbind entry points act on (pwpp_select_bound_call)
+  int scratch_slots = 0;                  // state / history slots after the streams' (the longest run of any bind), kept after unbind
   bool sets_on_device = false;            // the last call's sets were picked on the device (a stream table): range_fast asks every
                                           // set, and fetch_offsets fetches frame_set
 
@@ -405,15 +410,38 @@ int reserve_work(pwpp_ctx* ctx, int nframes, long long total, long long total_ch
   need(ctx->d_normals, nf * nb * 3);
   if (grow)
     return fail(PWPP_ERR_CAPACITY, "a call of " + std::to_string(nframes) + " frames and " + std::to_string(total) +
-                                       " points does not fit the work buffers frozen by the bound call (pwpp_unbind_call lifts the freeze)");
+                                       " points does not fit the work buffers frozen by the bound calls (unbinding every bound call lifts the freeze)");
   if (err != cudaSuccess) return fail(PWPP_ERR_CUDA, std::string("reserving the work buffers: ") + cudaGetErrorString(err));
+  return PWPP_OK;
+}
+
+bool any_bound(const pwpp_ctx* ctx) {
+  for (const pwpp_ctx::Bound& b : ctx->bound)
+    if (b.on) return true;
+  return false;
+}
+
+// A bind (nframes > 0: frames, total points, chunks) or a stream-table enable (nframes = 0) that needs slots scratch slots, while
+// another bound call has run or been captured: its graphs hold the work and state buffers, so neither may move.
+// PWPP_ERR_CAPACITY, before anything changes, when either would have to grow. With no run yet everything grows as needed.
+int check_growth(pwpp_ctx* ctx, int slots, int nframes = 0, long long total = 0, long long chunks = 0) {
+  bool ran = false;
+  for (const pwpp_ctx::Bound& b : ctx->bound) ran = ran || b.ran;
+  if (!ran) return PWPP_OK;
+  const std::string fix = ", and another bound call has run or been captured: bind every call, widest first, before the first run or capture";
+  if (slots > ctx->scratch_slots)
+    return fail(PWPP_ERR_CAPACITY, "the call needs " + std::to_string(slots) + " scratch state slots (its longest run), the ctx has " +
+                                       std::to_string(ctx->scratch_slots) + fix);
+  if (nframes > 0 && reserve_work(ctx, nframes, total, chunks, true, true))
+    return fail(PWPP_ERR_CAPACITY, "a call of " + std::to_string(nframes) + " frames and " + std::to_string(total) +
+                                       " points (the sum of max_n) needs larger work buffers" + fix);
   return PWPP_OK;
 }
 
 // A direct call while a call is bound: PWPP_ERR_CAPACITY, before anything runs or changes, when the call would grow a work
 // buffer. Frame f has n[f] points (negative sizes were refused by the caller).
 int check_frozen(pwpp_ctx* ctx, int nframes, const int64_t* n, bool with_input) {
-  if (!ctx->bound.on) return PWPP_OK;
+  if (!any_bound(ctx)) return PWPP_OK;
   long long total = 0, chunks = 0;
   for (int f = 0; f < nframes; ++f) {
     total += n[f];
@@ -473,7 +501,7 @@ int prepare_call(pwpp_ctx* ctx, int nframes, const int32_t* streams, cudaStream_
   CU_TRY(cudaEventRecord(ctx->tab_ev[tb], s));
   ctx->last_nframes = nframes;
   ctx->last_total = total;
-  ctx->last_bound = false;
+  ctx->last_call = -1;
   ctx->sets_on_device = false;
   ctx->counts_fetched = ctx->idx_fetched = ctx->patches_fetched = false;
   ctx->stage_valid = false;
@@ -877,10 +905,10 @@ int check_frame(pwpp_ctx* ctx, int f) {
   return PWPP_OK;
 }
 
-// The bound call's point offsets (the device scan of its accepted counts) into the host description of the last call, and with
-// a stream table the sets its frames ran with.
+// The last bound call's point offsets (the device scan of its accepted counts) into the host description of the last call, and
+// with a stream table the sets its frames ran with.
 int fetch_offsets(pwpp_ctx* ctx) {
-  if (!ctx->last_bound || ctx->off_fetched) return PWPP_OK;
+  if (ctx->last_call < 0 || ctx->off_fetched) return PWPP_OK;
   int rc = bind_device(ctx);
   if (rc) return rc;
   const int nf = ctx->last_nframes;
@@ -1461,16 +1489,16 @@ int pwpp_estimate_device_records(pwpp_ctx* ctx, int nframes, const int32_t* stre
 
 // ---- the bound call (include/pwpp.h) ----
 
-// Makes the bound call the ctx's last call, run on stream s: the host getters fetch its offsets first (fetch_offsets).
-static void make_bound_last(pwpp_ctx* ctx, cudaStream_t s) {
-  const pwpp_ctx::Bound& b = ctx->bound;
+// Makes bound call k the ctx's last call, run on stream s: the host getters fetch its offsets first (fetch_offsets).
+static void make_bound_last(pwpp_ctx* ctx, int k, cudaStream_t s) {
+  const pwpp_ctx::Bound& b = ctx->bound[k];
   ctx->last_nframes = b.nf;
   ctx->frame_set = b.frame_set;
   ctx->last_recs.clear();
   ctx->last_pts = ctx->d_in.p;
   ctx->last_stream = s;
   ctx->last_total = 0;
-  ctx->last_bound = true;
+  ctx->last_call = k;
   ctx->sets_on_device = b.d_streams != nullptr;
   ctx->off_fetched = ctx->counts_fetched = ctx->idx_fetched = ctx->patches_fetched = false;
   ctx->rec_gathered = ctx->rec_fetched = false;
@@ -1522,7 +1550,8 @@ static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
                           const int32_t* d_slots, const int64_t* d_offsets = nullptr, int64_t capacity = 0) {
   int rc = check_records_call(ctx, nframes, streams, frames, max_n, layouts);
   if (rc) return rc;
-  if (ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "a call is already bound (pwpp_unbind_call releases it)");
+  if (ctx->bound[ctx->sel].on)
+    return fail(PWPP_ERR_INVALID_ARG, "a call is already bound as bound call " + std::to_string(ctx->sel) + " (pwpp_unbind_call releases it)");
   if (!rings && !d_offsets && !d_counts) return fail(PWPP_ERR_INVALID_ARG, "d_counts is NULL");
   if (rings && (rc = check_rings(nframes, rings, max_n, layouts))) return rc;
   pwpp_ctx::Bound b;
@@ -1574,13 +1603,14 @@ static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
       }
     }
   }
+  if ((rc = check_growth(ctx, slots, nframes, b.cap_pt_off[nframes], chunks))) return rc;
   rc = bind_device(ctx);
   if (rc) return rc;
   // the buffers may move: whatever the ctx enqueued before has finished with them, and the last call's results end here
   if (ctx->last_stream) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
   CU_TRY(cudaStreamSynchronize(ctx->stream));
   ctx->last_nframes = 0;
-  ctx->last_bound = false;
+  ctx->last_call = -1;
   if (slots > ctx->scratch_slots) {
     // the streams' states and histories move with their contents; a failed allocation leaves them where they were
     const size_t ns = (size_t) ctx->num_streams + slots;
@@ -1634,7 +1664,7 @@ static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
   }
   CU_TRY(cudaDeviceSynchronize());
   b.on = true;
-  ctx->bound = std::move(b);
+  ctx->bound[ctx->sel] = std::move(b);
   return PWPP_OK;
 }
 
@@ -1669,21 +1699,22 @@ int pwpp_bind_call_packed(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
 // its capacities. Never through launch_range: its own capture would nest inside a caller's.
 int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (!ctx->bound[ctx->sel].on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   int rc = bind_device(ctx);
   if (rc) return rc;
   const auto t0 = std::chrono::steady_clock::now();
   cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
-  const pwpp_ctx::Bound& b = ctx->bound;
+  const int k = ctx->sel;   // a graph captured from here holds this call, whatever is selected later
+  pwpp_ctx::Bound& b = ctx->bound[k];
   const int nf = b.nf;
-  // the host-side description launch_range_impl reads (direct calls between runs replace it)
+  // the host-side description launch_range_impl reads (direct calls and other bound calls between runs replace it)
   ctx->last_nframes = nf;
   ctx->runs = b.runs;
   ctx->frame_set = b.frame_set;
   ctx->sets_on_device = b.d_streams != nullptr;
   ctx->chunk_off = b.cap_chunk_off;
   ctx->pt_off = b.cap_pt_off;
-  ctx->bound.ran = true;
+  b.ran = true;
   const BoundActions A{b.d_actions, b.d_bact.p, b.d_bscratch.p, b.d_bdep.p, ctx->d_states_init.p, ctx->d_states.p};
   const BoundStreams T{b.d_streams, b.d_bread.p, b.d_bclaim.p, b.d_bset_of.p, b.d_bruns.p, (int) b.runs.size() - 1, ctx->num_streams};
   const RecordFrame* recs = b.d_brec.p;   // the record table the unpack and the gather read
@@ -1782,7 +1813,7 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     }
     CU_TRY(cudaGetLastError());
   }
-  make_bound_last(ctx, s);
+  make_bound_last(ctx, k, s);
   ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
   return PWPP_OK;
 }
@@ -1790,20 +1821,20 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
 int pwpp_bound_call_results(pwpp_ctx* ctx, const int32_t** d_indices, const int64_t** d_offsets, const int32_t** d_num_ground,
                             const int32_t** d_status) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
-  make_bound_last(ctx, ctx->last_stream ? ctx->last_stream : ctx->stream);
+  if (!ctx->bound[ctx->sel].on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  make_bound_last(ctx, ctx->sel, ctx->last_stream ? ctx->last_stream : ctx->stream);
   if (d_indices) *d_indices = ctx->d_out_idx.p;
   if (d_offsets) *d_offsets = reinterpret_cast<const int64_t*>(ctx->d_pt_off.p);
   if (d_num_ground) *d_num_ground = ctx->d_counts.p;
-  if (d_status) *d_status = ctx->bound.d_bstatus.p;
+  if (d_status) *d_status = ctx->bound[ctx->sel].d_bstatus.p;
   return PWPP_OK;
 }
 
 int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call_rings)");
-  if (!ctx->bound.d_slots) return fail(PWPP_ERR_INVALID_ARG, "the bound call has no rings (pwpp_bind_call_rings)");
-  if (d_slots_read) *d_slots_read = ctx->bound.d_bslot.p;
+  if (!ctx->bound[ctx->sel].on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call_rings)");
+  if (!ctx->bound[ctx->sel].d_slots) return fail(PWPP_ERR_INVALID_ARG, "the bound call has no rings (pwpp_bind_call_rings)");
+  if (d_slots_read) *d_slots_read = ctx->bound[ctx->sel].d_bslot.p;
   return PWPP_OK;
 }
 
@@ -1812,7 +1843,7 @@ int pwpp_bound_call_slots(pwpp_ctx* ctx, const int32_t** d_slots_read) {
 // streams repeat). The tables are built in buffers of their own and moved into the bound call only when all of them exist.
 int pwpp_bind_stream_table(pwpp_ctx* ctx, const int32_t* d_streams) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  pwpp_ctx::Bound& b = ctx->bound;
+  pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (!d_streams) return fail(PWPP_ERR_INVALID_ARG, "d_streams is NULL");
   if (b.d_streams) return fail(PWPP_ERR_INVALID_ARG, "a stream table is already enabled for the bound call");
@@ -1830,6 +1861,7 @@ int pwpp_bind_stream_table(pwpp_ctx* ctx, const int32_t* d_streams) {
       dep[f] = r > 0;
     }
   }
+  if ((rc = check_growth(ctx, slots))) return rc;
   // the state buffers may move: whatever the ctx enqueued before has finished with them
   if (ctx->last_stream) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
   CU_TRY(cudaStreamSynchronize(ctx->stream));
@@ -1871,24 +1903,37 @@ int pwpp_bind_stream_table(pwpp_ctx* ctx, const int32_t* d_streams) {
 
 int pwpp_bound_call_streams(pwpp_ctx* ctx, const int32_t** d_streams_read) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
-  if (!ctx->bound.d_streams) return fail(PWPP_ERR_INVALID_ARG, "the bound call has no stream table (pwpp_bind_stream_table)");
-  if (d_streams_read) *d_streams_read = ctx->bound.d_bread.p;
+  if (!ctx->bound[ctx->sel].on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (!ctx->bound[ctx->sel].d_streams) return fail(PWPP_ERR_INVALID_ARG, "the bound call has no stream table (pwpp_bind_stream_table)");
+  if (d_streams_read) *d_streams_read = ctx->bound[ctx->sel].d_bread.p;
   return PWPP_OK;
 }
 
 int pwpp_unbind_call(pwpp_ctx* ctx) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  if (!ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound");
+  if (!ctx->bound[ctx->sel].on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound");
   int rc = bind_device(ctx);
   if (rc) return rc;
-  ctx->bound = pwpp_ctx::Bound();   // releases the bound call's buffers
+  ctx->bound[ctx->sel] = pwpp_ctx::Bound();   // releases the bound call's buffers; no shared buffer moves
   return PWPP_OK;
+}
+
+int pwpp_select_bound_call(pwpp_ctx* ctx, int k) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (k < 0 || k >= PWPP_MAX_BOUND_CALLS)
+    return fail(PWPP_ERR_INVALID_ARG, "bound call " + std::to_string(k) + " is outside [0, " + std::to_string(PWPP_MAX_BOUND_CALLS) + ")");
+  ctx->sel = k;
+  return PWPP_OK;
+}
+
+int pwpp_selected_bound_call(const pwpp_ctx* ctx) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  return ctx->sel;
 }
 
 int pwpp_bind_record_results(pwpp_ctx* ctx, int parts) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  pwpp_ctx::Bound& b = ctx->bound;
+  pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
   if (b.rec_parts) return fail(PWPP_ERR_INVALID_ARG, "record results are already enabled for the bound call");
@@ -1914,7 +1959,7 @@ int pwpp_bind_record_results(pwpp_ctx* ctx, int parts) {
 int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void** d_nonground, const int64_t** h_offsets,
                               const int32_t** d_counts) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  const pwpp_ctx::Bound& b = ctx->bound;
+  const pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (!b.rec_parts) return fail(PWPP_ERR_INVALID_ARG, "record results are not enabled for the bound call (pwpp_bind_record_results)");
   if (d_ground) *d_ground = (b.rec_parts & PWPP_PART_GROUND) ? b.d_bground.p : nullptr;
@@ -1926,7 +1971,7 @@ int pwpp_bound_record_results(pwpp_ctx* ctx, const void** d_ground, const void**
 
 int pwpp_bind_getter_results(pwpp_ctx* ctx, int what) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  pwpp_ctx::Bound& b = ctx->bound;
+  pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (what < 1 || what > 7) return fail(PWPP_ERR_INVALID_ARG, "what must be a non-empty set of PWPP_GETTER_GROUND_XYZ, PWPP_GETTER_NONGROUND_XYZ and PWPP_GETTER_STATE");
   if (b.getters) return fail(PWPP_ERR_INVALID_ARG, "getter results are already enabled for the bound call");
@@ -1965,7 +2010,7 @@ static int reserve_packed_offsets(pwpp_ctx::Bound& b) {
 
 int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  pwpp_ctx::Bound& b = ctx->bound;
+  pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
   if (b.packed_xyz) return fail(PWPP_ERR_INVALID_ARG, "packed xyz is already enabled for the bound call");
@@ -1984,7 +2029,7 @@ int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts) {
 
 int pwpp_bind_packed_records(pwpp_ctx* ctx, int parts) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  pwpp_ctx::Bound& b = ctx->bound;
+  pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
   if (b.packed_rec) return fail(PWPP_ERR_INVALID_ARG, "packed records are already enabled for the bound call");
@@ -2008,7 +2053,7 @@ int pwpp_bind_packed_records(pwpp_ctx* ctx, int parts) {
 int pwpp_bound_packed_records(pwpp_ctx* ctx, const void** d_ground, const void** d_nonground, const int64_t** d_ground_off,
                               const int64_t** d_nonground_off, int32_t* point_step) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  const pwpp_ctx::Bound& b = ctx->bound;
+  const pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (!b.packed_rec) return fail(PWPP_ERR_INVALID_ARG, "packed records are not enabled for the bound call (pwpp_bind_packed_records)");
   const bool g = b.packed_rec & PWPP_PART_GROUND, n = b.packed_rec & PWPP_PART_NONGROUND;
@@ -2023,7 +2068,7 @@ int pwpp_bound_packed_records(pwpp_ctx* ctx, const void** d_ground, const void**
 int pwpp_bound_packed_xyz(pwpp_ctx* ctx, const float** d_ground, const float** d_nonground, const int64_t** d_ground_off,
                           const int64_t** d_nonground_off) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  const pwpp_ctx::Bound& b = ctx->bound;
+  const pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (!b.packed_xyz) return fail(PWPP_ERR_INVALID_ARG, "packed xyz is not enabled for the bound call (pwpp_bind_packed_xyz)");
   const bool g = b.packed_xyz & PWPP_PART_GROUND, n = b.packed_xyz & PWPP_PART_NONGROUND;
@@ -2037,7 +2082,7 @@ int pwpp_bound_packed_xyz(pwpp_ctx* ctx, const float** d_ground, const float** d
 int pwpp_bound_getter_results(pwpp_ctx* ctx, pwpp_bound_getters* out) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (!out) return fail(PWPP_ERR_INVALID_ARG, "out is NULL");
-  const pwpp_ctx::Bound& b = ctx->bound;
+  const pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   *out = pwpp_bound_getters{};
   out->ground_xyz = (b.getters & PWPP_GETTER_GROUND_XYZ) ? b.d_bgxyz.p : nullptr;
@@ -2058,7 +2103,7 @@ int pwpp_bound_getter_results(pwpp_ctx* ctx, pwpp_bound_getters* out) {
 static int gather_records(pwpp_ctx* ctx) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (ctx->last_nframes <= 0) return fail(PWPP_ERR_INVALID_ARG, "no estimate call yet");
-  if (ctx->last_bound)
+  if (ctx->last_call >= 0)
     return fail(PWPP_ERR_INVALID_ARG, "record results are not available for a bound call (pwpp_run_bound_call): their gather needs host offsets (pwpp_bind_record_results gives a bound call its own)");
   if (ctx->last_recs.empty()) return fail(PWPP_ERR_INVALID_ARG, "the last estimate call did not take records (pwpp_estimate_host_records / pwpp_estimate_device_records)");
   if (ctx->rec_gathered) return PWPP_OK;
@@ -2354,7 +2399,7 @@ int pwpp_clone(const pwpp_ctx* src_c, int device, pwpp_ctx** out) {
   *out = nullptr;
   if (!src_c) return fail(PWPP_ERR_INVALID_ARG, "src is NULL");
   pwpp_ctx* src = const_cast<pwpp_ctx*>(src_c);   // fetching the last call's host description caches it; nothing observable changes
-  if (src->bound.on) return fail(PWPP_ERR_INVALID_ARG, "pwpp_clone: the source holds a bound call; pwpp_unbind_call first");
+  if (any_bound(src)) return fail(PWPP_ERR_INVALID_ARG, "pwpp_clone: the source holds a bound call; pwpp_unbind_call first");
   if (device < 0) device = src->device;
   int rc = bind_device(src);
   if (rc) return rc;
@@ -2418,7 +2463,7 @@ int pwpp_set_output_order(pwpp_ctx* ctx, int order) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (order != PWPP_ORDER_BIN && order != PWPP_ORDER_REFERENCE && order != PWPP_ORDER_REFERENCE_EXACT)
     return fail(PWPP_ERR_INVALID_ARG, "order must be PWPP_ORDER_BIN, PWPP_ORDER_REFERENCE or PWPP_ORDER_REFERENCE_EXACT");
-  if (ctx->bound.on) return fail(PWPP_ERR_INVALID_ARG, "the output order cannot change while a call is bound (it keeps the order it was bound with)");
+  if (any_bound(ctx)) return fail(PWPP_ERR_INVALID_ARG, "the output order cannot change while a call is bound (it keeps the order it was bound with)");
   if (order != ctx->order_mode) ++g_alloc_gen;   // captured graphs were recorded with the other launch sequence
   ctx->order_mode = order;
   return PWPP_OK;

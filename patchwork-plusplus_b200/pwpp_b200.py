@@ -89,6 +89,8 @@ def load_library():
     lib.pwpp_run_bound_call.argtypes = [vp, vp]; lib.pwpp_run_bound_call.restype = i32
     lib.pwpp_bound_call_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_bound_call_results.restype = i32
     lib.pwpp_unbind_call.argtypes = [vp]; lib.pwpp_unbind_call.restype = i32
+    lib.pwpp_select_bound_call.argtypes = [vp, i32]; lib.pwpp_select_bound_call.restype = i32
+    lib.pwpp_selected_bound_call.argtypes = [vp]; lib.pwpp_selected_bound_call.restype = i32
     lib.pwpp_bind_record_results.argtypes = [vp, i32]; lib.pwpp_bind_record_results.restype = i32
     lib.pwpp_bound_record_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     lib.pwpp_bound_record_results.restype = i32
@@ -154,6 +156,20 @@ def _check(rc):
         raise PwppError(f"pwpp error {rc}: {load_library().pwpp_last_error().decode()}")
 
 
+MAX_BOUND_CALLS = 32   # PWPP_MAX_BOUND_CALLS
+
+
+class _BoundCall:
+    """What the Engine keeps of one bound call of the ctx (pwpp_select_bound_call)."""
+
+    def __init__(self):
+        self.call = None            # (frames, counts, streams, sum of max_n) of the bind
+        self.actions = None         # its actions tensor (bind_call(actions=...)), kept alive while bound
+        self.rings = None           # its ring tensors and slots (bind_call_rings), kept alive while bound
+        self.streams = None         # its stream table (bind_stream_table), kept alive while bound
+        self.table_streams = None   # Engine._streams while its last run is the last call and it has a stream table
+
+
 class Engine:
     """One `pwpp_ctx`: `num_streams` independent sensor streams on one CUDA device.
 
@@ -186,10 +202,9 @@ class Engine:
         self._n = []
         self._streams = []   # stream of every frame of the last call
         self._rec_dtypes = []   # record dtype of every frame of the last records call (uint8 rows of point_step for (buffer, layout) frames)
-        self._bound = None      # (frames, counts, streams, sum of max_n) of the bound call
-        self._bound_actions = None   # its actions tensor (bind_call(actions=...)), kept alive while bound
-        self._bound_rings = None     # its ring tensors and slots (bind_call_rings), kept alive while bound
-        self._bound_streams = None   # its stream table (bind_stream_table), kept alive while bound
+        self._calls = [_BoundCall() for _ in range(MAX_BOUND_CALLS)]
+        self._sel = 0       # the selected bound call (select_bound_call)
+        self._last = None   # the _BoundCall that ran last (run_bound_call / bound_call_results)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -328,8 +343,8 @@ class Engine:
         else:
             _check(self.lib.pwpp_bind_call_actions(self._h, nf, ids.ctypes.data, p, n, lays, C.c_void_p(counts.data_ptr()),
                                                    C.c_void_p(actions.data_ptr())))
-        self._bound = (list(frames), counts, ids.tolist(), sum(int(k) for k in max_n))
-        self._bound_actions = actions
+        self._call.call = (list(frames), counts, ids.tolist(), sum(int(k) for k in max_n))
+        self._call.actions = actions
 
     def bind_call_rings(self, rings, max_n, layouts, slots, streams=None, actions=None):
         """Binds a call whose frames live in scan rings (pwpp_bind_call_rings): at every run or replay frame f reads slot
@@ -377,9 +392,9 @@ class Engine:
         lays = (PwppPointLayout * max(nf, 1))(*layouts)
         _check(self.lib.pwpp_bind_call_rings(self._h, nf, ids.ctypes.data, descs, n, lays, C.c_void_p(slots.data_ptr()),
                                              C.c_void_p(actions.data_ptr() if actions is not None else None)))
-        self._bound = ([r[0] for r in rings], None, ids.tolist(), sum(int(k) for k in max_n))
-        self._bound_actions = actions
-        self._bound_rings = (list(rings), slots)
+        self._call.call = ([r[0] for r in rings], None, ids.tolist(), sum(int(k) for k in max_n))
+        self._call.actions = actions
+        self._call.rings = (list(rings), slots)
 
     def bind_call_packed(self, points, offsets, max_n, layout=None, streams=None, actions=None):
         """Binds a call over one packed batch (pwpp_bind_call_packed): at every run or replay frame f is records
@@ -409,8 +424,8 @@ class Engine:
         n = (C.c_int64 * max(nf, 1))(*[int(k) for k in max_n])
         _check(self.lib.pwpp_bind_call_packed(self._h, nf, ids.ctypes.data, C.c_void_p(points.data_ptr()), C.byref(layout), capacity, n,
                                               C.c_void_p(offsets.data_ptr()), C.c_void_p(actions.data_ptr() if actions is not None else None)))
-        self._bound = ([points] * nf, offsets, ids.tolist(), sum(int(k) for k in max_n))
-        self._bound_actions = actions
+        self._call.call = ([points] * nf, offsets, ids.tolist(), sum(int(k) for k in max_n))
+        self._call.actions = actions
 
     def bind_packed_xyz(self, ground: bool = True, nonground: bool = True):
         """Enables packed xyz results for the bound call (pwpp_bind_packed_xyz): every later run_bound_call, and every graph
@@ -426,7 +441,7 @@ class Engine:
         import torch
         ptrs = [C.c_void_p() for _ in range(4)]
         _check(self.lib.pwpp_bound_packed_xyz(self._h, *[C.byref(p) for p in ptrs]))
-        nf, rows = len(self._bound[0]), self._bound[3]
+        nf, rows = len(self._call.call[0]), self._call.call[3]
 
         class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
             def __init__(self, ptr, shape, typestr):
@@ -460,7 +475,7 @@ class Engine:
         ptrs = [C.c_void_p() for _ in range(4)]
         step = C.c_int32()
         _check(self.lib.pwpp_bound_packed_records(self._h, *[C.byref(p) for p in ptrs], C.byref(step)))
-        nf, rows, step = len(self._bound[0]), self._bound[3], step.value
+        nf, rows, step = len(self._call.call[0]), self._call.call[3], step.value
 
         class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
             def __init__(self, ptr, shape, typestr):
@@ -483,7 +498,7 @@ class Engine:
         import torch
         a = C.c_void_p()
         _check(self.lib.pwpp_bound_call_slots(self._h, C.byref(a)))
-        nf = len(self._bound[0])
+        nf = len(self._call.call[0])
 
         class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
             def __init__(self, ptr, n):
@@ -496,14 +511,14 @@ class Engine:
         same stream is skipped with STREAM_OUT_OF_RANGE / STREAM_DUPLICATE. The runs stay those of the bound streams. Call it
         before the bound call's first run; the tensor is kept alive while bound and its contents may change between runs."""
         import torch
-        if self._bound is None:
+        if self._call.call is None:
             raise PwppError("no call is bound")
-        nf = len(self._bound[2])
+        nf = len(self._call.call[2])
         if not (isinstance(streams, torch.Tensor) and streams.is_cuda and streams.dtype == torch.int32 and streams.is_contiguous()
                 and streams.numel() == nf):
             raise PwppError(f"streams must be a contiguous int32 CUDA tensor of {nf} entries")
         _check(self.lib.pwpp_bind_stream_table(self._h, C.c_void_p(streams.data_ptr())))
-        self._bound_streams = streams
+        self._call.streams = streams
 
     def bound_call_streams(self):
         """Torch view (int32 [nframes]) of the streams the last run read (pwpp_bound_call_streams): the run's own copy, invalid ids
@@ -511,7 +526,7 @@ class Engine:
         import torch
         a = C.c_void_p()
         _check(self.lib.pwpp_bound_call_streams(self._h, C.byref(a)))
-        nf = len(self._bound[2])
+        nf = len(self._call.call[2])
 
         class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
             def __init__(self, ptr, n):
@@ -532,7 +547,7 @@ class Engine:
         a, b, c, d = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
         _check(self.lib.pwpp_bound_call_results(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
         self._use_bound()
-        frames, _, _, cap = self._bound
+        frames, _, _, cap = self._call.call
         nf = len(frames)
 
         class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
@@ -558,7 +573,7 @@ class Engine:
         import torch
         a, b, c, d = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
         _check(self.lib.pwpp_bound_record_results(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
-        nf = len(self._bound[0])
+        nf = len(self._call.call[0])
         off = np.ctypeslib.as_array((C.c_int64 * (nf + 1)).from_address(c.value)).copy()
         total = int(off[-1])
 
@@ -594,7 +609,7 @@ class Engine:
         import torch
         g = PwppBoundGetters()
         _check(self.lib.pwpp_bound_getter_results(self._h, C.byref(g)))
-        nf = len(self._bound[0])
+        nf = len(self._call.call[0])
         row_off = np.ctypeslib.as_array((C.c_int64 * (nf + 1)).from_address(g.h_row_off)).copy()
         rows, stride = int(row_off[-1]), int(g.patch_row_stride)
 
@@ -621,25 +636,47 @@ class Engine:
                 "n_flatness": view(s and s + PwppState.n_flatness.offset, (nf, 4), "<i4", (st, 4))}
 
     def unbind_call(self):
-        if self._bound_streams is not None and self._streams is getattr(self, "_table_streams", None):
+        """Releases the selected bound call (pwpp_unbind_call). When it ran last, the host getters keep serving its results."""
+        if self._streams is self._call.table_streams:
             # the last call keeps its host getters after the unbind: name the streams its frames read (an invalid id: the bound
             # stream, whose set the frame ran with), so bin_results sizes the records of each frame's set without the table
             self.synchronize()
             read = self.bound_call_streams().cpu().tolist()
-            self._streams = [s if 0 <= s < self.num_streams else b for s, b in zip(read, self._bound[2])]
-        self._table_streams = None
+            self._streams = [s if 0 <= s < self.num_streams else b for s, b in zip(read, self._call.call[2])]
         _check(self.lib.pwpp_unbind_call(self._h))
-        self._bound = None
-        self._bound_actions = None
-        self._bound_rings = None
-        self._bound_streams = None
+        self._calls[self._sel] = _BoundCall()
+
+    def select_bound_call(self, k: int):
+        """Selects bound call k of the ctx, 0 <= k < MAX_BOUND_CALLS (pwpp_select_bound_call): the bind, run, result and unbind
+        methods act on it. Host-only. Call 0 is selected at creation. A graph captured from run_bound_call holds the call that was
+        selected at capture. The calls share the streams, the scratch slots and the work buffers (include/pwpp.h)."""
+        _check(self.lib.pwpp_select_bound_call(self._h, int(k)))
+        self._sel = int(k)
+
+    @property
+    def selected_bound_call(self) -> int:
+        return self._sel
+
+    @property
+    def _call(self):
+        return self._calls[self._sel]
 
     def _use_bound(self):
-        """The host getters now serve the bound call: its frame sizes are fetched from the device when first needed."""
+        """The host getters now serve the selected bound call: its frame sizes are fetched from the device when first needed."""
         self._n = None
-        self._streams = list(self._bound[2])
+        self._streams = list(self._call.call[2])
         self._rec_dtypes = []
-        self._table_streams = self._streams if self._bound_streams is not None else None   # bin_results: sets read on the device
+        self._call.table_streams = self._streams if self._call.streams is not None else None   # bin_results: sets read on the device
+        self._last = self._call
+
+    def _last_call_streams(self):
+        """bound_call_streams of the call that ran last, whichever call is selected."""
+        sel = self._sel
+        self.select_bound_call(self._calls.index(self._last))
+        try:
+            return self.bound_call_streams()
+        finally:
+            self.select_bound_call(sel)
 
     def _sizes(self):
         """Point count of every frame of the last call (after a bound call: from its device offsets, one device->host copy)."""
@@ -745,12 +782,12 @@ class Engine:
 
     def bin_results(self, f=0):
         """Patch records of frame f of the last call: the bins of the frame's parameter set."""
-        if self._streams is getattr(self, "_table_streams", None):
+        if self._last is not None and self._streams is self._last.table_streams:
             # a stream table: the C-ABI writes the bins of the set the frame ran with; the stream it read names that set (an
             # invalid id: its bound stream's)
             arr = (PwppBinResult * self.nbins)()
             _check(self.lib.pwpp_copy_bin_results(self._h, f, C.byref(arr)))
-            s = int(self.bound_call_streams()[f])
+            s = int(self._last_call_streams()[f])
             nb = self.stream_num_bins(s if 0 <= s < self.num_streams else self._streams[f])
             return (PwppBinResult * nb).from_buffer(arr)
         nb = self.stream_num_bins(self._streams[f]) if 0 <= f < len(self._streams) else self.nbins   # (a bad f: the C-ABI reports it)
@@ -863,6 +900,7 @@ class Engine:
         e._h, e.device = h, self.device if device is None else int(device)
         e.params = list(self.params) if isinstance(self.params, list) else self.params
         e._n, e._streams, e._rec_dtypes = None if self._n is None else list(self._n), list(self._streams), []
+        e._calls, e._sel, e._last = [_BoundCall() for _ in range(MAX_BOUND_CALLS)], 0, None   # a clone holds no bound call
         return e
 
     def device_index_lists(self):
