@@ -661,6 +661,57 @@ int pwpp_unbind_call(pwpp_ctx* ctx);
 int pwpp_select_bound_call(pwpp_ctx* ctx, int k);
 int pwpp_selected_bound_call(const pwpp_ctx* ctx);
 
+/* ---- width ladders: the GPU picks how many positions a bound call launches, at every run or replay ----------------------------
+ * A scheduler kernel inside the caller's graph that picks the streams of a tick (a stream table) cannot tell the host how many
+ * sensors arrived without a device-to-host read, so it cannot pick one of several graphs. A width ladder lets one graph do it:
+ * at every run or replay the GPU reads the table kernel's status array and launches the call cut to the narrowest width of the
+ * ladder that holds every position that runs. A narrow width sizes every grid for the capacities of its first positions only.
+ * The kernel variants stay those of each run's full length: a 4-wide launch of a 64-frame run keeps the batch kernels, because
+ * the small-call kernels (PWPP_SMALL_CALL) give plane fits that differ from the batch kernels' in the last bits, which moves the
+ * adaptive thresholds, and a ladder changes no result.
+ *
+ * pwpp_bind_width_ladder: enables the ladder for the selected bound call. widths[0 .. nwidths) must be strictly increasing and
+ * each in [1, nframes); the call's own nframes is always the implicit last width, so 1 <= nwidths <= PWPP_MAX_LADDER_WIDTHS - 1.
+ * Host work that synchronizes: it captures the call's launch sequence cut
+ * at every width into graphs the call owns, so later result enables (pwpp_bind_record_results, pwpp_bind_getter_results,
+ * pwpp_bind_packed_xyz, pwpp_bind_packed_records) and pwpp_bind_stream_table on that call return PWPP_ERR_INVALID_ARG: enable
+ * them before the ladder. It grows no buffer, so it is allowed after runs and captures; graphs captured before it keep running
+ * without the ladder. Once enabled, the call counts as captured for the growth rule of "Several bound calls".
+ * PWPP_ERR_INVALID_ARG, with the call unchanged, when no call is bound, for bad widths (NULL, nwidths outside that range, not
+ * strictly increasing, outside [1, nframes)), for a second enable, and for a call with neither actions nor a
+ * stream table (every position of such a call runs, so the widest width would always be chosen). pwpp_unbind_call releases it.
+ *
+ * The width rule. A position RUNS when the table kernel leaves it status 0, PWPP_COUNT_OUT_OF_RANGE, PWPP_SLOT_OUT_OF_RANGE or
+ * PWPP_OFFSETS_OUT_OF_RANGE (frames whose stream state advances). It is REJECTED when its status is PWPP_FRAME_SKIPPED,
+ * PWPP_ACTION_INVALID, PWPP_STREAM_OUT_OF_RANGE or PWPP_STREAM_DUPLICATE. With L = 1 + the last position that runs (0 when none
+ * does), the run launches the smallest ladder width w >= max(L, 1). A scheduler that compacts the present streams to the
+ * front gets the narrow launch; one that leaves a present stream at the last position gets the full width.
+ *
+ * The contract: enabling a ladder changes no result. After every run or replay, everything equals, bit for bit, what the same
+ * call without a ladder gives after the same runs: the indices, offsets, num_ground, status and the read copies of streams,
+ * slots and actions; the record, getter (xyz and state rows), packed-xyz and packed-record buffers, including the bytes past
+ * every count, which stay unwritten; the patch rows; everything the host getters return (indices, xyz, centers, normals, bin
+ * results, bin ids, per-frame state); and the export blob of every stream. The positions at or past w are rejected frames: they
+ * still run, as the empty frames on their scratch slots that they are without a ladder, through the same kernels with grids
+ * sized for empty frames, and the gathers still cover all nframes positions.
+ *
+ * Graphs. A run on a stream that is capturing (global capture mode included) adds to the caller's graph the table kernel,
+ * k_ladder_select and one conditional SWITCH node whose bodies are copies of the prebuilt width graphs; an uncaptured run
+ * launches the same graph, built at enable time, as an executable graph the call owns. CUDA's rules for graphs that contain a
+ * conditional node apply to the caller's graph: it cannot be cloned, cannot be used as a child graph node, and one executable
+ * instance of it must not run twice at once. A caller that embeds its graph as a child graph uses the call without a ladder.
+ *
+ * pwpp_launch_count rises per run exactly as for the same call without a ladder, plus one for the selector, whatever width runs.
+ *
+ * pwpp_bound_call_width: host-only. *d_width is a device int32 at a fixed address while the call stays bound: the width the last
+ * run or replay launched. For a call without a ladder it holds nframes; a ladder enable sets it to 0 until its first run.
+ * PWPP_ERR_INVALID_ARG when no call is bound.
+ *
+ * Memory: 4 bytes of device memory per bound call for the width, and per ladder one graph per width. */
+#define PWPP_MAX_LADDER_WIDTHS 8
+int pwpp_bind_width_ladder(pwpp_ctx* ctx, int nwidths, const int32_t* widths);
+int pwpp_bound_call_width(pwpp_ctx* ctx, const int32_t** d_width);
+
 /* cudaDeviceSynchronize() on the ctx's device: what a binding calls before handing device memory produced on an unknown
  * stream to pwpp_estimate_device (and what makes its results visible to every stream afterwards). */
 int pwpp_device_synchronize(pwpp_ctx* ctx);

@@ -140,6 +140,12 @@ def build_examples(force=False):
     if force or _newer(out15, [src15] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
         subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
                                "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out15, src15])
+    # the width selector of bound calls with a width ladder, inside a real graph (GPU cases of tests/test_bound_ladder_backends.py)
+    src16 = os.path.join(REPO, "tests", "gpu_bound_ladder_probe.cu")
+    out16 = os.path.join(LIB, "libpwpp_bound_ladder_probe.so")
+    if force or _newer(out16, [src16] + glob.glob(os.path.join(HERE, "csrc", "*")) + [os.path.join(REPO, "include", "pwpp.h")]):
+        subprocess.check_call([NVCC, "-O3", "-std=c++17", "-lineinfo", *ARCH, "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared",
+                               "-I" + os.path.join(REPO, "include"), "-I" + os.path.join(HERE, "csrc"), "-cudart", "static", "-o", out16, src16])
     src14 = os.path.join(REPO, "tests", "pwpp_copy_driver.cpp")   # copies of the drop-in class against the real engine (GPU test)
     out14 = os.path.join(LIB, "pwpp_copy_driver")
     if force or _newer(out14, [src14, hdr, core]):

@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
@@ -20,6 +21,7 @@
 #include "pwpp_records.cuh"
 #include "pwpp_getters.cuh"
 #include "pwpp_state_copy.cuh"
+#include "pwpp_ladder.cuh"
 #include "pwpp_tuning.h"
 #include "pwpp_host.hpp"
 
@@ -142,6 +144,24 @@ struct FitLaunch {
 
 constexpr int NUM_SIDE = 6;
 
+// A bound call's width ladder (pwpp_bind_width_ladder): the selector's widths, one plain graph per width holding the call's launch
+// sequence cut at that width (enqueue_bound_body), and the whole run (table, selector, SWITCH node) as an executable graph for
+// runs on a stream that is not capturing.
+struct BoundLadder {
+  LadderWidths widths{};
+  std::vector<cudaGraph_t> bodies;
+  cudaGraphExec_t exec = nullptr;
+  long long body_launches = 0;   // launches of the widest body: the same call's count without a ladder, less the table kernel
+  long long launches = 0;        // launches of one run
+  BoundLadder() = default;
+  BoundLadder(const BoundLadder&) = delete;
+  BoundLadder& operator=(const BoundLadder&) = delete;
+  ~BoundLadder() {
+    if (exec) cudaGraphExecDestroy(exec);
+    for (cudaGraph_t g : bodies) cudaGraphDestroy(g);
+  }
+};
+
 struct pwpp_ctx {
   // parameter sets (pwpp_create: one) and the set of every stream; the kernels get the set records by value
   int num_sets = 1;
@@ -253,8 +273,7 @@ struct pwpp_ctx {
     bool on = false;
     int nf = 0, has_intensity = 0;
     const long long* d_counts = nullptr;    // the caller's device counts
-    long long unpack_gx = 0;                // grid.x of the unpack, from the capacities
-    std::vector<int> runs, frame_set, run_chunks, cap_chunk_off;   // run_chunks[r]: the run's largest ceil(max_n / CHUNK_PTS)
+    std::vector<int> runs, frame_set, cap_chunk_off;
     std::vector<long long> cap_pt_off;      // the capacity layout: sizes grids and picks the dense front end only
     DevBuf<long long, false> d_bmax;        // [F] max_n
     DevBuf<int, false> d_bstream, d_bpset;  // [F] the bound call's stream and set tables
@@ -262,7 +281,6 @@ struct pwpp_ctx {
     std::vector<RecordFrame> recs;          // its record table (host copy of d_brec)
     DevBuf<RecordFrame, false> d_brec;      // [F] its record table
     int rec_parts = 0;                      // record results (pwpp_bind_record_results): PWPP_PART_* bits, 0 = off
-    long long rec_gx = 0;                   // grid.x of k_gather_record_parts, from the capacities
     std::vector<long long> rec_part_off;    // [F+1] byte offsets of every frame's region in each part buffer
     DevBuf<unsigned char, false> d_bground, d_bnonground;   // its record results, one buffer per part (region f at rec_part_off[f])
     DevBuf<long long, false> d_bpart_off;   // [F+1] rec_part_off
@@ -278,7 +296,6 @@ struct pwpp_ctx {
     const long long* d_offsets = nullptr;   // the caller's device offsets (pwpp_bind_call_packed), NULL: not packed
     long long capacity = 0;                 // records at the packed buffer's base
     int getters = 0;                        // getter results (pwpp_bind_getter_results): PWPP_GETTER_* bits, 0 = off
-    long long xyz_gx = 0;                   // grid.x of k_gather_xyz_parts, from the capacities
     DevBuf<float, false> d_bgxyz, d_bngxyz;  // getter results: [sum(max_n)][3] ground / non-ground xyz, frame f from row cap_pt_off[f]
     DevBuf<long long, false> d_bxyz_off;    // [F+1] cap_pt_off
     DevBuf<int, false> d_xyz_counts;        // [F][2]: ground, non-ground xyz rows of every frame of the last run
@@ -295,6 +312,8 @@ struct pwpp_ctx {
     DevBuf<int, false> d_bset_of;           // [num_streams] stream_set, for the sets of the streams read on the device
     DevBuf<int, false> d_bruns;             // [runs + 1] runs, for the duplicate check run by run
     bool ran = false;                       // a run was enqueued or captured: the state buffers may no longer move
+    DevBuf<int, false> d_width;             // the width the last run launched (pwpp_bound_call_width)
+    std::unique_ptr<BoundLadder> ladder;    // its width ladder (pwpp_bind_width_ladder), NULL: none
   };
   // Bound calls 0 .. PWPP_MAX_BOUND_CALLS - 1. They share the stream states, the scratch slots and the work buffers, so a bind
   // may grow those only while none of them has run (check_growth).
@@ -526,14 +545,19 @@ bool range_fast(const pwpp_ctx* ctx, int f0, int nf) {
 // one stream (a run or part of one). A frame range is the same launch sequence over per-frame arrays offset by f0 (frame
 // tables hold absolute point / chunk positions), which is what lets pwpp_estimate_host pipeline chunks of frames against
 // their H2D / D2H copies. Stream state and histories are indexed by the stream table, never by the frame.
-int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int has_intensity, cudaStream_t s, bool prof, int chunks_override) {
+// The kernel variants (small-call kernels, dense front end, fp32 binning filter) are those of frames [vf0, vf0 + vnf), by default
+// the range itself: a width-ladder body launches parts of a run with the run's variants, whose results it must reproduce.
+int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int has_intensity, cudaStream_t s, bool prof, int chunks_override,
+                      int vf0 = -1, int vnf = 0) {
+  if (vnf <= 0) { vf0 = f0; vnf = nf; }
   int max_chunks = 0;
   for (int f = f0; f < f0 + nf; ++f) max_chunks = std::max(max_chunks, ctx->chunk_off[f + 1] - ctx->chunk_off[f]);
   if (chunks_override > 0) max_chunks = chunks_override;   // graph capture: grids sized for a range of frame sizes (surplus CTAs exit at once)
+  if (chunks_override < 0) max_chunks = 0;                 // frames the bound table kernel rejected: empty on every run
   const int nb = ctx->gs.nbs, nbp = ctx->nbp, nb_all = nb + PW_NUM_PSEUDO;   // strides of the per-frame bin arrays (the largest set)
   const int nframes = nf;
   FrameTable ft{ctx->d_pt_off.p + f0, ctx->d_chunk_off.p + f0, ctx->d_stream.p + f0, ctx->d_pset.p + f0};
-  const bool fast = range_fast(ctx, f0, nf);
+  const bool fast = range_fast(ctx, vf0, vnf);
   StreamState* states = ctx->d_states.p;
   double* hist = ctx->d_hist.p;
   int* bin_off = ctx->d_bin_off.p + (size_t) f0 * (nbp + 1);
@@ -554,13 +578,13 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
   // latency of the longest patch counts, so patches above 512 points go to the CTA-per-patch kernels, and one frame's cloud is
   // binned by ~30 independent CTAs (the three stand-alone kernels) rather than by the 8 CTAs of one cluster: both shorten
   // the longest kernel of a one-frame call.
-  const bool small_call = nframes <= ctx->small_call_frames;
+  const bool small_call = vnf <= ctx->small_call_frames;
   const FitLaunch* fitk = small_call ? ctx->fit_small : ctx->fit;
   if (ctx->sw_front && !small_call) {
     // one thread-block cluster per frame: binning, scan and stable scatter in one kernel (pwpp_front.cuh)
     if (nframes > 0) {
       // 64 warps per frame for KITTI-sized frames, 128 for dense ones (pwpp_front.cuh)
-      const long long mean_front = (ctx->pt_off[f0 + nf] - ctx->pt_off[f0]) / std::max(nf, 1);
+      const long long mean_front = (ctx->pt_off[vf0 + vnf] - ctx->pt_off[vf0]) / std::max(vnf, 1);
       const bool dense = mean_front > 400000 && ctx->front_dense_ok;
       const int nt = dense ? FC_THREADS_DENSE : FC_THREADS;
       const size_t sm_f = front_cluster_smem_bytes(nbp, nt);
@@ -1575,15 +1599,9 @@ static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
     if (layouts[f].offset[3] >= 0) b.has_intensity = 1;
     b.frame_set.push_back(ctx->stream_set[streams[f]]);
   }
-  b.unpack_gx = b.cap_pt_off[nframes] > 0 ? rec_grid_x(b.cap_pt_off.data(), recs.data(), nframes) : 0;
   b.recs = recs;
   split_runs(ctx, nframes, streams);
   b.runs = ctx->runs;
-  for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
-    int m = 0;
-    for (int f = b.runs[r]; f < b.runs[r + 1]; ++f) m = std::max(m, b.cap_chunk_off[f + 1] - b.cap_chunk_off[f]);
-    b.run_chunks.push_back(m);
-  }
   std::vector<int> scratch, dep;
   int slots = 0;   // the longest run
   if (d_actions) {
@@ -1647,6 +1665,8 @@ static int bind_call_impl(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
   CU_TRY(cudaMemcpy(b.d_bpset.p, b.frame_set.data(), (size_t) nframes * sizeof(int), cudaMemcpyHostToDevice));
   CU_TRY(cudaMemcpy(b.d_brec.p, recs.data(), (size_t) nframes * sizeof(RecordFrame), cudaMemcpyHostToDevice));
   CU_TRY(cudaMemset(b.d_bstatus.p, 0, (size_t) nframes * sizeof(int)));
+  CU_TRY(b.d_width.reserve(1));
+  CU_TRY(cudaMemcpy(b.d_width.p, &nframes, sizeof(int), cudaMemcpyHostToDevice));
   if (rings) {
     std::vector<BoundRing> ring(nframes);
     for (int f = 0; f < nframes; ++f)
@@ -1695,29 +1715,29 @@ int pwpp_bind_call_packed(pwpp_ctx* ctx, int nframes, const int32_t* streams, co
   return bind_call_impl(ctx, nframes, streams, frames.data(), max_n, layouts.data(), nullptr, d_actions, nullptr, nullptr, d_offsets, capacity);
 }
 
-// One table launch, one unpack launch (capacities with points), then every run through launch_range_impl with grids sized for
-// its capacities. Never through launch_range: its own capture would nest inside a caller's.
-int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
-  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
-  if (!ctx->bound[ctx->sel].on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
-  int rc = bind_device(ctx);
-  if (rc) return rc;
-  const auto t0 = std::chrono::steady_clock::now();
-  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
-  const int k = ctx->sel;   // a graph captured from here holds this call, whatever is selected later
-  pwpp_ctx::Bound& b = ctx->bound[k];
-  const int nf = b.nf;
-  // the host-side description launch_range_impl reads (direct calls and other bound calls between runs replace it)
-  ctx->last_nframes = nf;
+// An enable that changes what a run of bound call b launches, after its width ladder captured the launch sequences.
+static int check_no_ladder(const pwpp_ctx::Bound& b, const char* what) {
+  if (b.ladder)
+    return fail(PWPP_ERR_INVALID_ARG, std::string("the bound call has a width ladder, which captured its launch sequences: enable ") + what +
+                                          " before the width ladder (pwpp_bind_width_ladder)");
+  return PWPP_OK;
+}
+
+// The host-side description launch_range_impl reads for bound call b (direct calls and other bound calls between runs replace it).
+static void describe_bound(pwpp_ctx* ctx, const pwpp_ctx::Bound& b) {
+  ctx->last_nframes = b.nf;
   ctx->runs = b.runs;
   ctx->frame_set = b.frame_set;
   ctx->sets_on_device = b.d_streams != nullptr;
   ctx->chunk_off = b.cap_chunk_off;
   ctx->pt_off = b.cap_pt_off;
-  b.ran = true;
+}
+
+// The first kernel of every run of bound call b: its frame table from the counts, actions, slots, offsets and streams.
+static int enqueue_bound_table(pwpp_ctx* ctx, pwpp_ctx::Bound& b, cudaStream_t s) {
+  const int nf = b.nf;
   const BoundActions A{b.d_actions, b.d_bact.p, b.d_bscratch.p, b.d_bdep.p, ctx->d_states_init.p, ctx->d_states.p};
   const BoundStreams T{b.d_streams, b.d_bread.p, b.d_bclaim.p, b.d_bset_of.p, b.d_bruns.p, (int) b.runs.size() - 1, ctx->num_streams};
-  const RecordFrame* recs = b.d_brec.p;   // the record table the unpack and the gather read
   if (b.d_slots) {
     const BoundRings G{b.d_slots, b.d_bslot.p, b.d_bring.p, b.d_brec.p, b.d_brun.p};
     if (b.d_streams)
@@ -1729,7 +1749,6 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     else
       k_bound_table_rings<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
                                                    ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, G);
-    recs = b.d_brun.p;
   } else if (b.d_offsets) {
     const BoundPacked P{b.d_offsets, b.capacity, b.d_brec.p, b.d_brun.p};
     if (b.d_streams)
@@ -1741,7 +1760,6 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     else
       k_bound_table_packed<<<1, BT_THREADS, 0, s>>>(nf, b.d_bmax.p, b.d_bstream.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p,
                                                     ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p, P);
-    recs = b.d_brun.p;
   } else if (b.d_streams) {
     k_bound_table_streams<<<1, BT_THREADS, 0, s>>>(nf, b.d_counts, b.d_bmax.p, b.d_bpset.p, ctx->d_pt_off.p, ctx->d_chunk_off.p, ctx->d_stream.p,
                                                    ctx->d_pset.p, b.d_bstatus.p, A, T);
@@ -1753,36 +1771,59 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
                                            ctx->d_stream.p, ctx->d_pset.p, b.d_bstatus.p);
   }
   ++ctx->launches;
-  if (b.unpack_gx > 0) {
-    k_unpack_records<<<dim3((unsigned) b.unpack_gx, (unsigned) nf), REC_THREADS, 0, s>>>(recs, ctx->d_pt_off.p, ctx->d_in.p);
+  CU_TRY(cudaGetLastError());
+  return PWPP_OK;
+}
+
+// Everything a run of bound call b launches after its table kernel, cut at width w (1 <= w <= nf): the unpack, then per run the
+// reset, the launch sequence and the state rows, then the gathers. Every grid is sized from the capacities of positions [0, w).
+// A run's positions at or past w (all rejected when the width rule picked w) are launched as a second range of frames with grids
+// for empty frames; the gathers keep grid.y = nf, so those frames' counts come from the same code as without a ladder. With
+// w = nf this is the launch sequence of a call without a ladder, grids included. The host description must be b's (describe_bound).
+static int enqueue_bound_body(pwpp_ctx* ctx, pwpp_ctx::Bound& b, cudaStream_t s, int w) {
+  const int nf = b.nf;
+  const RecordFrame* recs = (b.d_slots || b.d_offsets) ? b.d_brun.p : b.d_brec.p;   // the record table the unpack and the gathers read
+  const long long* cap = b.cap_pt_off.data();
+  if (cap[w] > 0) {
+    k_unpack_records<<<dim3((unsigned) rec_grid_x(cap, b.recs.data(), w), (unsigned) w), REC_THREADS, 0, s>>>(recs, ctx->d_pt_off.p, ctx->d_in.p);
     ++ctx->launches;
   }
   CU_TRY(cudaGetLastError());
   for (size_t r = 0; r + 1 < b.runs.size(); ++r) {
+    const int f0 = b.runs[r], f1 = b.runs[r + 1], cut = std::min(f1, std::max(f0, w));
     // the RESET frames whose stream ran in an earlier run; with a stream table the host cannot know which, so every RESET frame
     // of every later run (its dep is 1) is reset right before its run, from the streams the run read
     if (b.d_actions && (b.d_streams ? r > 0 : b.reset_run[r])) {
-      k_bound_reset<<<1, BR_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bact.p, b.d_bdep.p, b.d_streams ? b.d_bread.p : b.d_bstream.p,
+      k_bound_reset<<<1, BR_THREADS, 0, s>>>(f0, f1, b.d_bact.p, b.d_bdep.p, b.d_streams ? b.d_bread.p : b.d_bstream.p,
                                              ctx->d_states_init.p, ctx->d_states.p);
       ++ctx->launches;
       CU_TRY(cudaGetLastError());
     }
-    rc = launch_range_impl(ctx, b.runs[r], b.runs[r + 1] - b.runs[r], ctx->d_in.p, b.has_intensity, s, false, b.run_chunks[r]);
-    if (rc) return rc;
+    if (cut > f0) {
+      int chunks = 0;   // the largest ceil(max_n / CHUNK_PTS) of the range
+      for (int f = f0; f < cut; ++f) chunks = std::max(chunks, b.cap_chunk_off[f + 1] - b.cap_chunk_off[f]);
+      const int rc = launch_range_impl(ctx, f0, cut - f0, ctx->d_in.p, b.has_intensity, s, false, chunks, f0, f1 - f0);
+      if (rc) return rc;
+    }
+    if (f1 > cut) {
+      const int rc = launch_range_impl(ctx, cut, f1 - cut, ctx->d_in.p, b.has_intensity, s, false, -1, f0, f1 - f0);
+      if (rc) return rc;
+    }
     if (b.getters & PWPP_GETTER_STATE) {   // before a later run moves the run's streams
-      const int len = b.runs[r + 1] - b.runs[r];
+      const int len = f1 - f0;
       if (b.d_streams)
-        k_bound_states_streams<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bread.p, ctx->num_streams,
-                                                                                          ctx->d_states.p, b.d_bstates.p);
+        k_bound_states_streams<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(f0, f1, b.d_bread.p, ctx->num_streams, ctx->d_states.p,
+                                                                                          b.d_bstates.p);
       else
-        k_bound_states<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(b.runs[r], b.runs[r + 1], b.d_bstream.p, ctx->d_states.p, b.d_bstates.p);
+        k_bound_states<<<(len + BS_THREADS - 1) / BS_THREADS, BS_THREADS, 0, s>>>(f0, f1, b.d_bstream.p, ctx->d_states.p, b.d_bstates.p);
       ++ctx->launches;
       CU_TRY(cudaGetLastError());
     }
   }
+  const long long rec_gx = rec_parts_grid_x(cap, b.recs.data(), w), xyz_gx = xyz_parts_grid_x(cap, w);
   if (b.rec_parts) {   // the record results: both parts' lists are where the runs' k_emit left them
     const int first = b.rec_parts == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.rec_parts == 3 ? 2 : 1;
-    k_gather_record_parts<<<dim3((unsigned) b.rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
+    k_gather_record_parts<<<dim3((unsigned) rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
         recs, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_bpart_off.p, first, b.d_bground.p, b.d_bnonground.p,
         b.d_rec_counts.p);
     ++ctx->launches;
@@ -1790,7 +1831,7 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
   }
   if (b.getters & (PWPP_GETTER_GROUND_XYZ | PWPP_GETTER_NONGROUND_XYZ)) {   // the xyz of both lists, from the unpacked points
     const int parts = b.getters & 3, first = parts == PWPP_GETTER_NONGROUND_XYZ ? 1 : 0, nparts = parts == 3 ? 2 : 1;
-    k_gather_xyz_parts<<<dim3((unsigned) b.xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
+    k_gather_xyz_parts<<<dim3((unsigned) xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
         ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_bxyz_off.p, first, b.d_bgxyz.p, b.d_bngxyz.p,
         b.d_xyz_counts.p);
     ++ctx->launches;
@@ -1801,17 +1842,86 @@ int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
     ++ctx->launches;
     if (b.packed_xyz) {
       const int first = b.packed_xyz == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.packed_xyz == 3 ? 2 : 1;
-      k_gather_xyz_packed<<<dim3((unsigned) b.xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
+      k_gather_xyz_packed<<<dim3((unsigned) xyz_gx, (unsigned) nf, (unsigned) nparts), XYZ_THREADS, 0, s>>>(
           ctx->d_in.p, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_pg_off.p, b.d_png_off.p, first, b.d_pgxyz.p, b.d_pngxyz.p);
       ++ctx->launches;
     }
     if (b.packed_rec) {   // the records the runs read, as k_gather_record_parts reads them
       const int first = b.packed_rec == PWPP_PART_NONGROUND ? 1 : 0, nparts = b.packed_rec == 3 ? 2 : 1;
-      k_gather_record_packed<<<dim3((unsigned) b.rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
+      k_gather_record_packed<<<dim3((unsigned) rec_gx, (unsigned) nf, (unsigned) nparts), REC_THREADS, 0, s>>>(
           recs, ctx->d_pt_off.p, ctx->d_counts.p, nf, ctx->d_out_idx.p, b.d_pg_off.p, b.d_png_off.p, first, b.d_prec_g.p, b.d_prec_ng.p);
       ++ctx->launches;
     }
     CU_TRY(cudaGetLastError());
+  }
+  return PWPP_OK;
+}
+
+// A laddered run of bound call b into the graph that s is capturing: the table kernel, k_ladder_select, and a SWITCH node whose
+// body i is a child graph node holding a copy of L.bodies[i]. Conditional bodies may hold child graphs but no event nodes, which
+// is why the bodies (whose fit kernels fork to the side streams) are captured beforehand, outside any caller's capture.
+static int enqueue_ladder(pwpp_ctx* ctx, pwpp_ctx::Bound& b, const BoundLadder& L, cudaStream_t s) {
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  cudaGraph_t g = nullptr;
+  CU_TRY(cudaStreamGetCaptureInfo_v3(s, &st, nullptr, &g));
+  if (st != cudaStreamCaptureStatusActive) return fail(PWPP_ERR_CUDA, "the stream's capture was invalidated");
+  cudaGraphConditionalHandle h;
+  CU_TRY(cudaGraphConditionalHandleCreate(&h, g, 0, cudaGraphCondAssignDefault));
+  int rc = enqueue_bound_table(ctx, b, s);
+  if (rc) return rc;
+  k_ladder_select<<<1, LS_THREADS, 0, s>>>(b.nf, b.d_bstatus.p, L.widths, b.d_width.p, h);
+  ++ctx->launches;
+  CU_TRY(cudaGetLastError());
+  const cudaGraphNode_t* deps = nullptr;
+  const cudaGraphEdgeData* edges = nullptr;
+  size_t ndeps = 0;
+  CU_TRY(cudaStreamGetCaptureInfo_v3(s, &st, nullptr, &g, &deps, &edges, &ndeps));
+  cudaGraphNodeParams p = {};
+  p.type = cudaGraphNodeTypeConditional;
+  p.conditional.handle = h;
+  p.conditional.type = cudaGraphCondTypeSwitch;
+  p.conditional.size = (unsigned) L.widths.n;
+  cudaGraphNode_t node;
+  CU_TRY(cudaGraphAddNode_v2(&node, g, deps, edges, ndeps, &p));
+  for (int i = 0; i < L.widths.n; ++i) {
+    cudaGraphNode_t child;
+    CU_TRY(cudaGraphAddChildGraphNode(&child, p.conditional.phGraph_out[i], nullptr, 0, L.bodies[i]));
+  }
+  CU_TRY(cudaStreamUpdateCaptureDependencies_v2(s, &node, nullptr, 1, cudaStreamSetCaptureDependencies));
+  ctx->launches += L.body_launches;
+  return PWPP_OK;
+}
+
+// One table launch, then the body: one unpack launch (capacities with points), every run through launch_range_impl with grids
+// sized for its capacities, and the gathers. Never through launch_range: its own capture would nest inside a caller's. With a
+// width ladder the body is the SWITCH node of enqueue_ladder: captured into the caller's graph when s is capturing, otherwise
+// launched as the ladder's own executable graph.
+int pwpp_run_bound_call(pwpp_ctx* ctx, void* cuda_stream) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!ctx->bound[ctx->sel].on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  const auto t0 = std::chrono::steady_clock::now();
+  cudaStream_t s = cuda_stream ? (cudaStream_t) cuda_stream : ctx->stream;
+  const int k = ctx->sel;   // a graph captured from here holds this call, whatever is selected later
+  pwpp_ctx::Bound& b = ctx->bound[k];
+  describe_bound(ctx, b);
+  b.ran = true;
+  if (b.ladder) {
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    CU_TRY(cudaStreamIsCapturing(s, &st));
+    if (st != cudaStreamCaptureStatusNone) {
+      rc = enqueue_ladder(ctx, b, *b.ladder, s);
+      if (rc) return rc;
+    } else {
+      CU_TRY(cudaGraphLaunch(b.ladder->exec, s));
+      ctx->launches += b.ladder->launches;
+    }
+  } else {
+    rc = enqueue_bound_table(ctx, b, s);
+    if (rc) return rc;
+    rc = enqueue_bound_body(ctx, b, s, b.nf);
+    if (rc) return rc;
   }
   make_bound_last(ctx, k, s);
   ctx->last_time_us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
@@ -1846,10 +1956,12 @@ int pwpp_bind_stream_table(pwpp_ctx* ctx, const int32_t* d_streams) {
   pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (!d_streams) return fail(PWPP_ERR_INVALID_ARG, "d_streams is NULL");
+  int rc = check_no_ladder(b, "the stream table");
+  if (rc) return rc;
   if (b.d_streams) return fail(PWPP_ERR_INVALID_ARG, "a stream table is already enabled for the bound call");
   if (b.ran)
     return fail(PWPP_ERR_INVALID_ARG, "the bound call has run or been captured: enable its stream table before its first run (the state buffers may grow)");
-  int rc = bind_device(ctx);
+  rc = bind_device(ctx);
   if (rc) return rc;
   const int nf = b.nf, nruns = (int) b.runs.size() - 1, ns = ctx->num_streams;
   std::vector<int> scratch(nf), dep(nf);
@@ -1918,6 +2030,102 @@ int pwpp_unbind_call(pwpp_ctx* ctx) {
   return PWPP_OK;
 }
 
+// One plain graph per width, each captured on the ctx's own stream outside any caller's capture (the body forks to the side
+// streams), then the whole run (enqueue_ladder) captured once more into the executable graph of uncaptured runs. The host
+// description and the launch counter are the ctx's again afterwards: the enable is no run.
+int pwpp_bind_width_ladder(pwpp_ctx* ctx, int nwidths, const int32_t* widths) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
+  if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (b.ladder) return fail(PWPP_ERR_INVALID_ARG, "a width ladder is already enabled for the bound call");
+  if (!b.d_actions && !b.d_streams)
+    return fail(PWPP_ERR_INVALID_ARG, "the bound call has neither actions nor a stream table: every position runs, so the ladder would always pick the full width");
+  if (!widths) return fail(PWPP_ERR_INVALID_ARG, "widths is NULL");
+  if (nwidths < 1 || nwidths > PWPP_MAX_LADDER_WIDTHS - 1)
+    return fail(PWPP_ERR_INVALID_ARG, "nwidths must be in [1, " + std::to_string(PWPP_MAX_LADDER_WIDTHS - 1) + "] (nframes is the implicit last width)");
+  auto L = std::make_unique<BoundLadder>();
+  for (int i = 0; i < nwidths; ++i) {
+    if (widths[i] < 1 || widths[i] >= b.nf || (i > 0 && widths[i] <= widths[i - 1]))
+      return fail(PWPP_ERR_INVALID_ARG, "widths[" + std::to_string(i) + "] = " + std::to_string(widths[i]) +
+                                            ": widths must be strictly increasing and in [1, nframes = " + std::to_string(b.nf) + ")");
+    L->widths.w[i] = widths[i];
+  }
+  L->widths.w[nwidths] = b.nf;
+  L->widths.n = nwidths + 1;
+  int rc = bind_device(ctx);
+  if (rc) return rc;
+  if (ctx->last_stream) CU_TRY(cudaStreamSynchronize(ctx->last_stream));
+  CU_TRY(cudaStreamSynchronize(ctx->stream));
+  const int saved_nframes = ctx->last_nframes;
+  const std::vector<int> saved_runs = ctx->runs, saved_set = ctx->frame_set, saved_chunk = ctx->chunk_off;
+  const std::vector<long long> saved_pt = ctx->pt_off;
+  const bool saved_dev = ctx->sets_on_device;
+  const float4* saved_pts = ctx->last_pts;
+  const cudaStream_t saved_stream = ctx->last_stream;
+  const long long saved_launches = ctx->launches;
+  // a failed capture ends it here (cudaStreamEndCapture) and leaves its partial graph to L
+  auto capture = [&](cudaGraph_t* out, auto&& enqueue) -> int {
+    cudaStream_t s = ctx->stream;
+    CU_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    const int rc = enqueue(s);
+    const cudaError_t e = cudaStreamEndCapture(s, out);
+    if (rc) return rc;
+    CU_TRY(e);
+    return PWPP_OK;
+  };
+  auto build = [&]() -> int {
+    describe_bound(ctx, b);
+    for (int i = 0; i < L->widths.n; ++i) {
+      const long long l0 = ctx->launches;
+      cudaGraph_t g = nullptr;
+      const int rc = capture(&g, [&](cudaStream_t s) { return enqueue_bound_body(ctx, b, s, L->widths.w[i]); });
+      if (g) L->bodies.push_back(g);
+      if (rc) return rc;
+      L->body_launches = ctx->launches - l0;   // the last one, nframes wide, stays
+    }
+    const long long l0 = ctx->launches;
+    cudaGraph_t g = nullptr;
+    int rc = capture(&g, [&](cudaStream_t s) { return enqueue_ladder(ctx, b, *L, s); });
+    if (rc == PWPP_OK) {
+      const cudaError_t e = cudaGraphInstantiate(&L->exec, g, 0);
+      if (e != cudaSuccess) {
+        L->exec = nullptr;
+        rc = fail(PWPP_ERR_CUDA, std::string("instantiating the width ladder's graph: ") + cudaGetErrorString(e));
+      }
+    }
+    if (g) cudaGraphDestroy(g);
+    if (rc) return rc;
+    L->launches = ctx->launches - l0;
+    CU_TRY(cudaMemset(b.d_width.p, 0, sizeof(int)));
+    CU_TRY(cudaDeviceSynchronize());
+    return PWPP_OK;
+  };
+  rc = build();
+  ctx->last_nframes = saved_nframes;
+  ctx->runs = saved_runs;
+  ctx->frame_set = saved_set;
+  ctx->chunk_off = saved_chunk;
+  ctx->pt_off = saved_pt;
+  ctx->sets_on_device = saved_dev;
+  ctx->last_pts = saved_pts;
+  ctx->last_stream = saved_stream;
+  ctx->launches = saved_launches;
+  if (rc) {
+    cudaGetLastError();
+    return rc;
+  }
+  b.ladder = std::move(L);
+  b.ran = true;   // its graphs hold the shared buffers: no later bind may grow them
+  return PWPP_OK;
+}
+
+int pwpp_bound_call_width(pwpp_ctx* ctx, const int32_t** d_width) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (!ctx->bound[ctx->sel].on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
+  if (d_width) *d_width = ctx->bound[ctx->sel].d_width.p;
+  return PWPP_OK;
+}
+
 int pwpp_select_bound_call(pwpp_ctx* ctx, int k) {
   if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
   if (k < 0 || k >= PWPP_MAX_BOUND_CALLS)
@@ -1936,8 +2144,10 @@ int pwpp_bind_record_results(pwpp_ctx* ctx, int parts) {
   pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
+  int rc = check_no_ladder(b, "record results");
+  if (rc) return rc;
   if (b.rec_parts) return fail(PWPP_ERR_INVALID_ARG, "record results are already enabled for the bound call");
-  int rc = bind_device(ctx);
+  rc = bind_device(ctx);
   if (rc) return rc;
   const int nf = b.nf;
   std::vector<long long> off(nf + 1);   // the direct call's region layout with n = max_n
@@ -1951,7 +2161,6 @@ int pwpp_bind_record_results(pwpp_ctx* ctx, int parts) {
   CU_TRY(cudaMemset(b.d_rec_counts.p, 0, 2 * (size_t) nf * sizeof(int)));
   CU_TRY(cudaDeviceSynchronize());
   b.rec_part_off = std::move(off);
-  b.rec_gx = rec_parts_grid_x(b.cap_pt_off.data(), b.recs.data(), nf);
   b.rec_parts = parts;
   return PWPP_OK;
 }
@@ -1974,8 +2183,10 @@ int pwpp_bind_getter_results(pwpp_ctx* ctx, int what) {
   pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (what < 1 || what > 7) return fail(PWPP_ERR_INVALID_ARG, "what must be a non-empty set of PWPP_GETTER_GROUND_XYZ, PWPP_GETTER_NONGROUND_XYZ and PWPP_GETTER_STATE");
+  int rc = check_no_ladder(b, "getter results");
+  if (rc) return rc;
   if (b.getters) return fail(PWPP_ERR_INVALID_ARG, "getter results are already enabled for the bound call");
-  int rc = bind_device(ctx);
+  rc = bind_device(ctx);
   if (rc) return rc;
   const int nf = b.nf;
   const size_t rows = (size_t) std::max<long long>(b.cap_pt_off[nf], 1);
@@ -1992,7 +2203,6 @@ int pwpp_bind_getter_results(pwpp_ctx* ctx, int what) {
     CU_TRY(cudaMemset(b.d_bstates.p, 0, (size_t) nf * sizeof(pwpp_state)));
   }
   CU_TRY(cudaDeviceSynchronize());
-  b.xyz_gx = xyz_parts_grid_x(b.cap_pt_off.data(), nf);
   b.getters = what;
   return PWPP_OK;
 }
@@ -2013,8 +2223,10 @@ int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts) {
   pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
+  int rc = check_no_ladder(b, "packed xyz");
+  if (rc) return rc;
   if (b.packed_xyz) return fail(PWPP_ERR_INVALID_ARG, "packed xyz is already enabled for the bound call");
-  int rc = bind_device(ctx);
+  rc = bind_device(ctx);
   if (rc) return rc;
   const int nf = b.nf;
   const size_t rows = (size_t) std::max<long long>(b.cap_pt_off[nf], 1);
@@ -2022,7 +2234,6 @@ int pwpp_bind_packed_xyz(pwpp_ctx* ctx, int parts) {
   if (parts & PWPP_PART_NONGROUND) CU_TRY(b.d_pngxyz.reserve(3 * rows));
   if ((rc = reserve_packed_offsets(b))) return rc;
   CU_TRY(cudaDeviceSynchronize());
-  b.xyz_gx = xyz_parts_grid_x(b.cap_pt_off.data(), nf);
   b.packed_xyz = parts;
   return PWPP_OK;
 }
@@ -2032,20 +2243,21 @@ int pwpp_bind_packed_records(pwpp_ctx* ctx, int parts) {
   pwpp_ctx::Bound& b = ctx->bound[ctx->sel];
   if (!b.on) return fail(PWPP_ERR_INVALID_ARG, "no call is bound (pwpp_bind_call)");
   if (parts < 1 || parts > 3) return fail(PWPP_ERR_INVALID_ARG, "parts must be PWPP_PART_GROUND, PWPP_PART_NONGROUND or both");
+  int rc = check_no_ladder(b, "packed records");
+  if (rc) return rc;
   if (b.packed_rec) return fail(PWPP_ERR_INVALID_ARG, "packed records are already enabled for the bound call");
   const int nf = b.nf;
   for (int f = 1; f < nf; ++f)   // one step for the whole buffer: each part is one (rows, point_step) byte array
     if (b.recs[f].step != b.recs[0].step)
       return fail(PWPP_ERR_UNSUPPORTED, "frame " + std::to_string(f) + " has point_step " + std::to_string(b.recs[f].step) + ", frame 0 has " +
                                             std::to_string(b.recs[0].step) + ": packed records need one point_step (pwpp_bind_record_results does not)");
-  int rc = bind_device(ctx);
+  rc = bind_device(ctx);
   if (rc) return rc;
   const size_t bytes = (size_t) std::max<long long>(b.cap_pt_off[nf], 1) * (size_t) b.recs[0].step;
   if (parts & PWPP_PART_GROUND) CU_TRY(b.d_prec_g.reserve(bytes));
   if (parts & PWPP_PART_NONGROUND) CU_TRY(b.d_prec_ng.reserve(bytes));
   if ((rc = reserve_packed_offsets(b))) return rc;
   CU_TRY(cudaDeviceSynchronize());
-  b.rec_gx = rec_parts_grid_x(b.cap_pt_off.data(), b.recs.data(), nf);
   b.packed_rec = parts;
   return PWPP_OK;
 }

@@ -91,6 +91,8 @@ def load_library():
     lib.pwpp_unbind_call.argtypes = [vp]; lib.pwpp_unbind_call.restype = i32
     lib.pwpp_select_bound_call.argtypes = [vp, i32]; lib.pwpp_select_bound_call.restype = i32
     lib.pwpp_selected_bound_call.argtypes = [vp]; lib.pwpp_selected_bound_call.restype = i32
+    lib.pwpp_bind_width_ladder.argtypes = [vp, i32, vp]; lib.pwpp_bind_width_ladder.restype = i32
+    lib.pwpp_bound_call_width.argtypes = [vp, C.POINTER(vp)]; lib.pwpp_bound_call_width.restype = i32
     lib.pwpp_bind_record_results.argtypes = [vp, i32]; lib.pwpp_bind_record_results.restype = i32
     lib.pwpp_bound_record_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     lib.pwpp_bound_record_results.restype = i32
@@ -157,6 +159,7 @@ def _check(rc):
 
 
 MAX_BOUND_CALLS = 32   # PWPP_MAX_BOUND_CALLS
+MAX_LADDER_WIDTHS = 8  # PWPP_MAX_LADDER_WIDTHS
 
 
 class _BoundCall:
@@ -532,6 +535,28 @@ class Engine:
             def __init__(self, ptr, n):
                 self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<i4", "data": (ptr, False), "version": 3, "strides": None}
         return torch.as_tensor(_View(a.value, nf), device="cuda")
+
+    def bind_width_ladder(self, widths):
+        """Lets the GPU pick, at every run or replay, how many positions the bound call launches (pwpp_bind_width_ladder): the
+        narrowest of `widths` (strictly increasing, each in [1, nframes); nframes is always the last width) that holds every
+        position its table kernel did not reject. Results are bit for bit those of the call without a ladder. The call needs
+        actions or a stream table; enable result buffers and the stream table first. Host work that synchronizes."""
+        if self._call.call is None:
+            raise PwppError("no call is bound")
+        w = np.ascontiguousarray(widths, dtype=np.int32)
+        _check(self.lib.pwpp_bind_width_ladder(self._h, len(w), w.ctypes.data))
+
+    def bound_call_width(self):
+        """Torch view (int32 [1]) of the width the last run launched (pwpp_bound_call_width): nframes without a ladder, 0 after
+        the ladder's enable until its first run. Fixed address while the call is bound."""
+        import torch
+        a = C.c_void_p()
+        _check(self.lib.pwpp_bound_call_width(self._h, C.byref(a)))
+
+        class _View:   # __cuda_array_interface__ v3: torch.as_tensor wraps the memory without copying
+            def __init__(self, ptr):
+                self.__cuda_array_interface__ = {"shape": (1,), "typestr": "<i4", "data": (ptr, False), "version": 3, "strides": None}
+        return torch.as_tensor(_View(a.value), device="cuda")
 
     def run_bound_call(self, stream: int = 0):
         """Enqueues the bound call on CUDA stream `stream` (0: the ctx's own stream; inside torch.cuda.graph pass
