@@ -78,6 +78,8 @@ struct Params {
 
 // order inside a bin of the index lists (PatchWorkpp::setOutputOrder; the values are pwpp.h's PWPP_ORDER_*)
 enum class OutputOrder : int { Bin = PWPP_ORDER_BIN, Reference = PWPP_ORDER_REFERENCE, ReferenceExact = PWPP_ORDER_REFERENCE_EXACT };
+// arithmetic of the plane fits and of A-GLE (PatchWorkpp::setArithmetic; the values are pwpp.h's PWPP_ARITH_*)
+enum class Arithmetic : int { Double = PWPP_ARITH_DOUBLE, Reference = PWPP_ARITH_REFERENCE };
 
 class PatchWorkpp {
  public:
@@ -222,6 +224,9 @@ class PatchWorkpp {
   // ReferenceExact: the reference's order with equal z where libstdc++'s std::sort leaves them, so the lists equal the
   // unmodified reference's whenever the label sets do (pwpp.h, PWPP_ORDER_REFERENCE_EXACT)
   void setOutputOrder(OutputOrder order) { check(pwpp_set_output_order(ctx_, static_cast<int>(order))); }
+  // Double (default): order-free double sums; Reference: the reference's fp32 arithmetic, so that every getter returns the CPU
+  // library's values bit for bit (pwpp.h, PWPP_ARITH_REFERENCE)
+  void setArithmetic(Arithmetic arith) { check(pwpp_set_arithmetic(ctx_, static_cast<int>(arith))); }
 
   pwpp_ctx* handle() { return ctx_; }
 

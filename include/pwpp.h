@@ -643,7 +643,7 @@ int pwpp_unbind_call(pwpp_ctx* ctx);
  *     (d_indices, d_offsets, d_num_ground of pwpp_bound_call_results) and the patch rows of pwpp_bound_getter_results live in
  *     the work buffers: they hold the last run of any call (or the last direct call).
  *   - Growth. A bind may need larger work buffers (sum(max_n) points, nframes frames; under PWPP_ORDER_REFERENCE_EXACT also the
- *     fix-up's scratch) and a bind with actions or a stream-table enable more scratch slots. Before any bound call has run or
+ *     fix-up's scratch, under PWPP_ARITH_REFERENCE the fit scratch) and a bind with actions or a stream-table enable more scratch slots. Before any bound call has run or
  *     been captured they grow as needed. Afterwards captured graphs hold them, so such a bind or enable returns
  *     PWPP_ERR_CAPACITY before anything changes; the message names the points and frames or the scratch slots it needs. To
  *     avoid it, bind every call, widest shape first (each buffer then grows once), and enable its tables before the first run
@@ -775,6 +775,43 @@ int pwpp_set_output_order(pwpp_ctx* ctx, int order);
  * tie in z inside one part (their libstdc++ order simulated), out[1] = segments sorted by the depth-limit heap sort, out[2] =
  * bins holding a NaN z (std::sort run literally in one thread). Synchronises the device; reset != 0 zeroes them afterwards. */
 int pwpp_order_exact_counts(pwpp_ctx* ctx, uint64_t out[3], int reset);
+
+/* Arithmetic of the plane fits and of A-GLE (pwpp_set_arithmetic; the default is PWPP_ARITH_DOUBLE).
+ *   PWPP_ARITH_DOUBLE     the reference's formulas in IEEE double with order-free sums and a closed-form eigen solve: index
+ *                         SETS equal the reference's except where fp32 rounding decides a point (DESIGN.md section 3).
+ *   PWPP_ARITH_REFERENCE  the reference's own arithmetic (S:47-75, S:217-223, S:551-554), so every result is the reference
+ *                         build's bit for bit, patches of 1-4 points, collinear and vertical patches included:
+ *       - every plane fit sums its point set sequentially in fp32 in the z-sorted order of the bin (mean: 3 sums divided by
+ *         (float) n; covariance: 6 sums of (q_i - mean_i) * (q_j - mean_j) divided by (float) (double) (n - 1)), then runs the
+ *         fp32 two-sided Jacobi SVD with the sign flip of the normal; d = -(x0 + (x1 + x2)) in fp32. Every operation is
+ *         separately rounded. The point sets are the reference's subsequences of the sorted bin (R-VPF seeds and kept points,
+ *         R-GPF seeds and each round's kept points). Equal z follow the output order's build: under PWPP_ORDER_BIN and
+ *         PWPP_ORDER_REFERENCE ascending point index (std::stable_sort: results bit for bit libpwref_stable.so's), under
+ *         PWPP_ORDER_REFERENCE_EXACT the order libstdc++'s std::sort leaves them in (results bit for bit the unmodified
+ *         reference's, libpwref.so). So in a bin with equal z the output order can change the planes, and with them the
+ *         labels, in the low bits where the two builds differ;
+ *       - the point-plane distance is ((n0 x + n1 y) + n2 z) in fp32 plus d in double; the LPR height is the double sum of
+ *         at most num_lpr floats in sorted order;
+ *       - A-GLE reads the fp32 plane: flatness is the fp32 minimum of the singular values, line_variable the fp32 quotient
+ *         sv0 / sv1 and heading the double sum of fp32 products mean_i * normal_i. The thresholds, sensor_height and the
+ *         histories follow from the same sequential double sums as in the default mode;
+ *       - patch records, centers and normals hold the float values (widened where the record is double). TGR's double exp
+ *         may differ from glibc's in the last bit; it only feeds the > 0.5 revert test.
+ *     Unchanged: the two defined deviations (history bound, patches without a plane), non-finite z, RNR, binning and the
+ *     gate. pwpp_launch_count rises exactly as in the default mode (one fit kernel per patch-size class, one k_gle).
+ *     A fit of the reference mode costs sequential fp32 chains over its point set: the largest patch of a call bounds its
+ *     fit stage (DESIGN.md section 3 gives the measured cost). Memory: the work buffers of the mode grow by 46 bytes per point
+ *     of the call (sort keys 16, staged points 16, fit set 12, flags 2), the storage of the patches above 512 / 2048 points
+ *     that do not fit the fit kernels' shared memory, each patch at its own offset (about 5.5 GB for a call of 120 M points);
+ *     a bind in this mode reserves them as well.
+ * Rules, as for pwpp_set_output_order: refused (PWPP_ERR_INVALID_ARG) while any call is bound, so a captured graph keeps the
+ * arithmetic it was bound with; pwpp_clone copies it; stream-state blobs have one format in both modes and move between
+ * them. Switching back to PWPP_ARITH_DOUBLE gives exactly the results of a context that never left it.
+ * pwpp_arithmetic returns the context's mode (PWPP_ERR_INVALID_ARG for a NULL ctx). */
+#define PWPP_ARITH_DOUBLE 0
+#define PWPP_ARITH_REFERENCE 1
+int pwpp_set_arithmetic(pwpp_ctx* ctx, int arith);
+int pwpp_arithmetic(const pwpp_ctx* ctx);
 
 /* Host-side zero-copy view of the index lists of the last call (batch consumers: the per-frame getters above copy each
  * list once more, which for a 1024-frame batch is 0.5 GB of host memcpy): *h_indices -> the page-locked int32 buffer the

@@ -141,6 +141,12 @@ struct FitLaunch {
   int grid = 0, threads = 0;
   size_t smem = 0;
 };
+typedef void (*Ref32Kernel)(const float4*, FrameTable, const StreamState*, GeometrySets, AlgoParamSets, const int*, WorkQueues, int*, BinFit*, Ref32Scratch, int);
+struct Ref32Launch {
+  Ref32Kernel fn = nullptr;
+  int grid = 0, threads = 0;
+  size_t smem = 0;
+};
 
 constexpr int NUM_SIDE = 6;
 
@@ -215,6 +221,13 @@ struct pwpp_ctx {
   DevBuf<unsigned> d_ox_scratch;  // PWPP_ORDER_REFERENCE_EXACT only: workspace of the fix-up above 512 points, OX_X_WORDS words per point
   DevBuf<unsigned long long> d_ox_counts;   // [OX_NUM_STATS] counters of the fix-up (pwpp_order_exact_counts)
   int order_mode = 0;             // PWPP_ORDER_*
+  int arith = PWPP_ARITH_DOUBLE;  // PWPP_ARITH_*: the fit kernels and the k_gle instantiation of launch_range_impl
+  Ref32Launch fit_ref32[NUM_CLASSES];   // k_fit_ref32 of every patch-size class (PWPP_ARITH_REFERENCE)
+  // PWPP_ARITH_REFERENCE only: storage of the patches above the shared capacity of their k_fit_ref32 (Ref32Scratch)
+  DevBuf<unsigned long long> d_r32_keys;
+  DevBuf<float4> d_r32_pts;
+  DevBuf<float> d_r32_sel;
+  DevBuf<unsigned char> d_r32_flags;
   FitLaunch fit[NUM_CLASSES];   // persistent fit kernel of every patch-size class (variant chosen in pwpp_create)
   FitLaunch fit_small[NUM_CLASSES];   // the same for calls of at most small_call_frames frames (one CTA per patch above 512 points)
   int max_sectors = 0;
@@ -324,7 +337,7 @@ struct pwpp_ctx {
                                           // set, and fetch_offsets fetches frame_set
 
   // small calls (the reference's one-frame-per-call pattern): the launch sequence replayed as a CUDA graph
-  struct GraphKey { int nf, call_frames, has_intensity, chunks, fast; unsigned long long gen; const void* pts; };
+  struct GraphKey { int nf, call_frames, has_intensity, chunks, fast, arith; unsigned long long gen; const void* pts; };
   cudaGraphExec_t gexec[2] = {nullptr, nullptr};
   GraphKey gkey[2] = {};
   long long glaunches[2] = {0, 0};
@@ -420,6 +433,12 @@ int reserve_work(pwpp_ctx* ctx, int nframes, long long total, long long total_ch
   need(ctx->d_part, np);
   if (ctx->order_mode) need(ctx->d_labels, np);
   if (ctx->order_mode == PWPP_ORDER_REFERENCE_EXACT) need(ctx->d_ox_scratch, (size_t) OX_X_WORDS * std::max<size_t>(np, 1));
+  if (ctx->arith == PWPP_ARITH_REFERENCE) {
+    need(ctx->d_r32_keys, 2 * std::max<size_t>(np, 1));
+    need(ctx->d_r32_pts, std::max<size_t>(np, 1));
+    need(ctx->d_r32_sel, 3 * std::max<size_t>(np, 1));
+    need(ctx->d_r32_flags, 2 * std::max<size_t>(np, 1));
+  }
   need(ctx->d_fits, nf * nb);
   need(ctx->d_segs, nf * nb_all);
   for (int c = 0; c < NUM_CLASSES; ++c) need(ctx->d_wq_items[c], nf * nb);
@@ -633,6 +652,16 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
   // of CTAs per class that find their queue empty and, worse, keep the six classes from running side by side: cap the grid
   // by what the call can hold (a frame has at most a few hundred patches)
   auto launch_fit = [&](int c, cudaStream_t st) {
+    if (ctx->arith == PWPP_ARITH_REFERENCE) {   // the reference's fp32 fits (pwpp_fit_ref32.cuh), the same grid rule
+      const Ref32Launch& k = ctx->fit_ref32[c];
+      const Ref32Scratch scr{ctx->d_r32_keys.p, ctx->d_r32_pts.p, ctx->d_r32_sel.p, ctx->d_r32_flags.p};
+      const long long cap = (long long) nframes * (k.threads <= 128 ? 96 : 48);
+      const int grid = (int) std::min<long long>(k.grid, std::max<long long>(1, cap));
+      k.fn<<<grid, k.threads, k.smem, st>>>(ctx->d_sorted.p, ft, states, ctx->gs, ctx->aps, bin_off, wq, ctx->d_part.p, fits, scr,
+                                            ctx->order_mode == PWPP_ORDER_REFERENCE_EXACT ? 1 : 0);
+      ++ctx->launches;
+      return;
+    }
     const FitLaunch& k = fitk[c];
     if (!k.fn) return;
     const long long cap = (long long) nframes * (k.threads <= 128 ? 96 : 48);
@@ -708,7 +737,10 @@ int launch_range_impl(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int ha
   int* d_nd = ctx->d_counts.p + 2 * call_frames + f0;
   {
     const size_t gle_smem = gle_smem_bytes(ctx->max_sectors);
-    k_gle<<<nframes, 32, gle_smem, s>>>(ft, states, hist, ctx->hist_stride, ctx->gs, ctx->aps, nbp, ctx->max_sectors, bin_off, fits, segs, d_ng, d_np, centers, normals, d_nd);
+    if (ctx->arith == PWPP_ARITH_REFERENCE)
+      k_gle<true><<<nframes, 32, gle_smem, s>>>(ft, states, hist, ctx->hist_stride, ctx->gs, ctx->aps, nbp, ctx->max_sectors, bin_off, fits, segs, d_ng, d_np, centers, normals, d_nd);
+    else
+      k_gle<false><<<nframes, 32, gle_smem, s>>>(ft, states, hist, ctx->hist_stride, ctx->gs, ctx->aps, nbp, ctx->max_sectors, bin_off, fits, segs, d_ng, d_np, centers, normals, d_nd);
     ++ctx->launches;
   }
   STAGE_MARK();
@@ -740,9 +772,9 @@ int launch_range(pwpp_ctx* ctx, int f0, int nf, const float4* d_pts, int has_int
   for (int f = 0; f < nf; ++f) max_chunks = std::max(max_chunks, ctx->chunk_off[f + 1] - ctx->chunk_off[f]);
   const int capc = std::max(8, (max_chunks + 7) & ~7);
   const int slot = has_intensity ? 1 : 0;
-  const pwpp_ctx::GraphKey key{nf, ctx->last_nframes, has_intensity, capc, range_fast(ctx, 0, nf) ? 1 : 0, g_alloc_gen, (const void*) d_pts};
+  const pwpp_ctx::GraphKey key{nf, ctx->last_nframes, has_intensity, capc, range_fast(ctx, 0, nf) ? 1 : 0, ctx->arith, g_alloc_gen, (const void*) d_pts};
   pwpp_ctx::GraphKey& have = ctx->gkey[slot];
-  if (!ctx->gexec[slot] || have.nf != key.nf || have.call_frames != key.call_frames || have.chunks != key.chunks || have.fast != key.fast || have.gen != key.gen ||
+  if (!ctx->gexec[slot] || have.nf != key.nf || have.call_frames != key.call_frames || have.chunks != key.chunks || have.fast != key.fast || have.arith != key.arith || have.gen != key.gen ||
       have.pts != key.pts) {
     if (ctx->gexec[slot]) { cudaGraphExecDestroy(ctx->gexec[slot]); ctx->gexec[slot] = nullptr; }
     const long long l0 = ctx->launches;
@@ -1175,8 +1207,25 @@ static int create_impl(const pwpp_params* sets, int num_sets, const int32_t* str
         ctx->exact_k[q].smem = sm;
       }
     }
+    // reference arithmetic: one CTA per patch, 128 threads up to 512 points, 256 up to 4096 and 512 above, shared capacity 512 / 2048
+    // points (larger patches in the global scratch)
+    {
+      const size_t sm_s = ref32_smem_bytes(R32_SMALL_CAP), sm_b = ref32_smem_bytes(R32_BIG_CAP);
+      ctx->fit_ref32[0] = {k_fit_ref32<0, 128, R32_SMALL_CAP>, 0, 128, sm_s};
+      ctx->fit_ref32[1] = {k_fit_ref32<1, 128, R32_SMALL_CAP>, 0, 128, sm_s};
+      ctx->fit_ref32[2] = {k_fit_ref32<2, 256, R32_BIG_CAP>, 0, 256, sm_b};
+      ctx->fit_ref32[3] = {k_fit_ref32<3, 256, R32_BIG_CAP>, 0, 256, sm_b};
+      ctx->fit_ref32[4] = {k_fit_ref32<4, 512, R32_BIG_CAP>, 0, 512, sm_b};
+      ctx->fit_ref32[5] = {k_fit_ref32<5, 512, R32_BIG_CAP>, 0, 512, sm_b};
+      for (Ref32Launch& k : ctx->fit_ref32) {
+        if (k.smem > 48 * 1024) CU_TRY_CTX(raise_smem_limit(k.fn, k.smem));
+        int per_sm = 1;
+        CU_TRY_CTX(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, k.threads, k.smem));
+        k.grid = std::max(1, per_sm) * prop.multiProcessorCount;
+      }
+    }
     const size_t gle_smem = gle_smem_bytes(max_sectors);
-    if (gle_smem > 48 * 1024) CU_TRY_CTX(raise_smem_limit(k_gle, gle_smem));
+    if (gle_smem > 48 * 1024) { CU_TRY_CTX(raise_smem_limit(k_gle<false>, gle_smem)); CU_TRY_CTX(raise_smem_limit(k_gle<true>, gle_smem)); }
   }
   {
     const size_t scat = (size_t) (CHUNK_THREADS / 32) * ctx->nbp * sizeof(unsigned int);
@@ -2629,6 +2678,7 @@ int pwpp_clone(const pwpp_ctx* src_c, int device, pwpp_ctx** out) {
   const int sd = src->device;
   cudaStream_t s = c->stream;
   c->order_mode = src->order_mode;
+  c->arith = src->arith;
 #define CU_CLONE(expr) do { const cudaError_t _e = (expr); if (_e != cudaSuccess) return done(fail(PWPP_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e))); } while (0)
   // the point capacity of src's per-point buffers
   CU_CLONE(c->d_in.reserve(src->d_in.cap));
@@ -2680,6 +2730,17 @@ int pwpp_set_output_order(pwpp_ctx* ctx, int order) {
   ctx->order_mode = order;
   return PWPP_OK;
 }
+
+int pwpp_set_arithmetic(pwpp_ctx* ctx, int arith) {
+  if (!ctx) return fail(PWPP_ERR_INVALID_ARG, "ctx is NULL");
+  if (arith != PWPP_ARITH_DOUBLE && arith != PWPP_ARITH_REFERENCE) return fail(PWPP_ERR_INVALID_ARG, "arith must be PWPP_ARITH_DOUBLE or PWPP_ARITH_REFERENCE");
+  if (any_bound(ctx)) return fail(PWPP_ERR_INVALID_ARG, "the arithmetic cannot change while a call is bound (it keeps the arithmetic it was bound with)");
+  if (arith != ctx->arith) ++g_alloc_gen;   // captured graphs were recorded with the other fit kernels
+  ctx->arith = arith;
+  return PWPP_OK;
+}
+
+int pwpp_arithmetic(const pwpp_ctx* ctx) { return ctx ? ctx->arith : PWPP_ERR_INVALID_ARG; }
 
 int pwpp_order_exact_counts(pwpp_ctx* ctx, uint64_t out[3], int reset) {
   if (!ctx || !out) return fail(PWPP_ERR_INVALID_ARG, "ctx or out is NULL");

@@ -24,6 +24,7 @@
 #include "pwpp_fit.cuh"
 #include "pwpp_fit_big.cuh"
 #include "pwpp_fit_patch.cuh"
+#include "pwpp_fit_ref32.cuh"
 #include "pwpp_order.cuh"
 #include "pwpp_order_exact.cuh"
 #include "pwpp_front.cuh"
@@ -300,6 +301,10 @@ __host__ __device__ inline size_t gle_smem_bytes(int max_sectors) { return (size
 
 // hist_stride is the row stride of the histories (the largest history_cap of the sets); the logical capacity of a stream's rows
 // is its own set's history_cap, exactly as in a context created with that set alone. max_sectors sizes the shared memory.
+// Ref32 (reference arithmetic, pwpp_set_arithmetic): the patch records hold float values, and S:217-223 reads them as the
+// reference does: line_variable is the fp32 quotient sv0 / sv1 and heading sums fp32 products. (The flatness, the fp32
+// minimum of the singular values, is the same value as the double minimum of the widened floats.)
+template <bool Ref32 = false>
 __global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restrict__ states, double* __restrict__ hist, int hist_stride,
                                             const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps, int nbp, int max_sectors, const int* __restrict__ bin_off, BinFit* __restrict__ fits, BinSeg* __restrict__ segs,
                                             int* __restrict__ num_ground, int* __restrict__ num_patches, float* __restrict__ centers, float* __restrict__ normals,
@@ -416,10 +421,16 @@ __global__ void __launch_bounds__(32) k_gle(FrameTable ft, StreamState* __restri
         double ground_flatness = v[6];
         if (v[7] < ground_flatness) ground_flatness = v[7];
         if (v[8] < ground_flatness) ground_flatness = v[8];
-        const double line_variable = v[7] != 0 ? ddiv(v[6], v[7]) : DBL_MAX;
-        double heading = 0.0;
+        double line_variable, heading = 0.0;
+        if constexpr (Ref32) {
+          line_variable = v[7] != 0 ? (double) fdiv((float) v[6], (float) v[7]) : DBL_MAX;
 #pragma unroll
-        for (int k = 0; k < 3; ++k) heading = dadd(heading, dmul(v[k], v[3 + k]));
+          for (int k = 0; k < 3; ++k) heading = dadd(heading, (double) fmul((float) v[k], (float) v[3 + k]));
+        } else {
+          line_variable = v[7] != 0 ? ddiv(v[6], v[7]) : DBL_MAX;
+#pragma unroll
+          for (int k = 0; k < 3; ++k) heading = dadd(heading, dmul(v[k], v[3 + k]));
+        }
         const bool is_upright = ground_uprightness > ap.uprightness_thr;
         const bool is_heading_outside = heading < 0.0;
         bool is_not_elevated = false, is_flat = false;

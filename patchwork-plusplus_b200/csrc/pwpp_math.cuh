@@ -78,6 +78,20 @@ PW_HD float fsqrt(float a) {
   return sqrtf(a);
 #endif
 }
+PW_HD float fsub(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+PW_HD float fdiv(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fdiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
 
 // Smallest float >= t (NaN stays NaN). For every float z, ±inf and NaN included:  (double) z < t  <=>  z < float_ru(t).
 // If float_ru(t) == t both sides compare the same value. Otherwise no float lies in [t, float_ru(t)), so a float is
@@ -366,6 +380,112 @@ PW_HD void jacobi_svd3(double cxx, double cxy, double cxz, double cyy, double cy
   }
   sv[0] = s0; sv[1] = s1; sv[2] = s2;
   ucol2[0] = c2[0]; ucol2[1] = c2[1]; ucol2[2] = c2[2];
+}
+
+// ---- the reference's own fp32 Jacobi SVD (reference arithmetic, pwpp_set_arithmetic) -----------------------
+// Two-sided Jacobi SVD of a 3x3 matrix in float, the algorithm published for Eigen 3.4.0's JacobiSVD that S:62 runs,
+// every operation rounded separately. W and U are column-major (M(i,j) = M[i + 3 * j]); sv comes out descending and U's
+// columns follow it. A non-finite entry gives U = I and NaN singular values (S:57 on one point divides 0 by 0).
+// x_i <- c x_i + s y_i ; y_i <- -s x_i + c y_i for the three entries x = M[x0 + i * inc], y = M[y0 + i * inc]
+PW_HD void rot3f(float* M, int x0, int y0, int inc, float c, float s) {
+  if (c == 1.f && s == 0.f) return;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const float xi = M[x0 + i * inc], yi = M[y0 + i * inc];
+    M[x0 + i * inc] = fadd(fmul(c, xi), fmul(s, yi));
+    M[y0 + i * inc] = fadd(-fmul(s, xi), fmul(c, yi));
+  }
+}
+PW_HD void jacobi_svd3f(const float cov[9], float sv[3], float U[9]) {
+  const float precision = 2.f * FLT_EPSILON, considerAsZero = FLT_MIN;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) U[k] = (k % 4 == 0) ? 1.f : 0.f;
+  float scale = 0.f;
+  bool finite = true;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    const float v = fabsf(cov[k]);
+    if (!(v <= FLT_MAX)) finite = false;
+    if (v > scale) scale = v;
+  }
+  if (!finite) { sv[0] = sv[1] = sv[2] = NAN; return; }
+  if (scale == 0.f) scale = 1.f;
+  float W[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) W[k] = fdiv(cov[k], scale);
+  float maxDiag = 0.f;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) { const float v = fabsf(W[4 * i]); if (v > maxDiag) maxDiag = v; }
+  bool finished = false;
+  while (!finished) {
+    finished = true;
+#pragma unroll
+    for (int pq = 0; pq < 3; ++pq) {
+      const int p = pq == 0 ? 1 : 2, q = pq == 2 ? 1 : 0;   // (1,0), (2,0), (2,1)
+      float thr = fmul(precision, maxDiag);
+      if (considerAsZero > thr) thr = considerAsZero;
+      if (fabsf(W[p + 3 * q]) > thr || fabsf(W[q + 3 * p]) > thr) {
+        finished = false;
+        // the 2x2 block made symmetric by one rotation (real_2x2_jacobi_svd)
+        float m00 = W[p + 3 * p], m01 = W[p + 3 * q], m10 = W[q + 3 * p], m11 = W[q + 3 * q];
+        float r1c, r1s;
+        const float t = fadd(m00, m11), dd = fsub(m10, m01);
+        if (fabsf(dd) < FLT_MIN) { r1s = 0.f; r1c = 1.f; }
+        else { const float u = fdiv(t, dd); const float tmp = fsqrt(fadd(1.f, fmul(u, u))); r1s = fdiv(1.f, tmp); r1c = fdiv(u, tmp); }
+        if (!(r1c == 1.f && r1s == 0.f)) {
+          const float a00 = fadd(fmul(r1c, m00), fmul(r1s, m10)), a10 = fadd(-fmul(r1s, m00), fmul(r1c, m10));
+          const float a01 = fadd(fmul(r1c, m01), fmul(r1s, m11)), a11 = fadd(-fmul(r1s, m01), fmul(r1c, m11));
+          m00 = a00; m10 = a10; m01 = a01; m11 = a11;
+        }
+        // j_right.makeJacobi(m00, m01, m11)
+        float jrc, jrs;
+        const float deno = fmul(2.f, fabsf(m01));
+        if (deno < FLT_MIN) { jrc = 1.f; jrs = 0.f; }
+        else {
+          const float tau = fdiv(fsub(m00, m11), deno);
+          const float w = fsqrt(fadd(fmul(tau, tau), 1.f));
+          const float tn = tau > 0.f ? fdiv(1.f, fadd(tau, w)) : fdiv(1.f, fsub(tau, w));
+          const float sign_t = tn > 0.f ? 1.f : -1.f;
+          const float nn = fdiv(1.f, fsqrt(fadd(fmul(tn, tn), 1.f)));
+          jrs = fmul(fmul(fmul(-sign_t, fdiv(m01, fabsf(m01))), fabsf(tn)), nn);
+          jrc = nn;
+        }
+        // j_left = rot1 * j_right^T
+        const float oc = jrc, os = -jrs;
+        const float jlc = fsub(fmul(r1c, oc), fmul(r1s, os)), jls = fadd(fmul(r1c, os), fmul(r1s, oc));
+        rot3f(W, p, q, 3, jlc, jls);           // W.applyOnTheLeft(p, q, j_left): rows p, q
+        rot3f(U, 3 * p, 3 * q, 1, jlc, jls);   // U.applyOnTheRight(p, q, j_left^T): columns p, q
+        rot3f(W, 3 * p, 3 * q, 1, jrc, -jrs);  // W.applyOnTheRight(p, q, j_right): columns p, q
+        const float a1 = fabsf(W[p + 3 * p]), a2 = fabsf(W[q + 3 * q]);
+        const float mx = a1 > a2 ? a1 : a2;
+        if (mx > maxDiag) maxDiag = mx;
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const float a = W[4 * i];
+    sv[i] = fabsf(a);
+    if (a < 0.f) { U[3 * i] = -U[3 * i]; U[3 * i + 1] = -U[3 * i + 1]; U[3 * i + 2] = -U[3 * i + 2]; }
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) sv[i] = fmul(sv[i], scale);
+  // selection sort, descending, the first maximal position wins; U's columns move along
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    int pos = 0;
+    float mx = sv[i];
+#pragma unroll
+    for (int k = 1; k < 3 - i; ++k) if (sv[i + k] > mx) { mx = sv[i + k]; pos = k; }
+    if (mx == 0.f) break;
+#pragma unroll
+    for (int c = i + 1; c < 3; ++c)   // the swap with constant indices, so that sv and U stay in registers
+      if (pos == c - i) {
+        const float ts = sv[i]; sv[i] = sv[c]; sv[c] = ts;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { const float tu = U[k + 3 * i]; U[k + 3 * i] = U[k + 3 * c]; U[k + 3 * c] = tu; }
+      }
+  }
 }
 
 // ---- closed-form symmetric 3x3 eigen-solver ----------------------------------------------------------------

@@ -72,6 +72,8 @@ def load_library():
     lib.pwpp_stage_name.argtypes = [i32]; lib.pwpp_stage_name.restype = C.c_char_p
     lib.pwpp_launch_count.argtypes = [vp]; lib.pwpp_launch_count.restype = i64
     lib.pwpp_set_output_order.argtypes = [vp, i32]; lib.pwpp_set_output_order.restype = i32
+    lib.pwpp_set_arithmetic.argtypes = [vp, i32]; lib.pwpp_set_arithmetic.restype = i32
+    lib.pwpp_arithmetic.argtypes = [vp]; lib.pwpp_arithmetic.restype = i32
     lib.pwpp_order_exact_counts.argtypes = [vp, vp, i32]; lib.pwpp_order_exact_counts.restype = i32
     lib.pwpp_host_results.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]; lib.pwpp_host_results.restype = i32
     lib.pwpp_bind_host_to_device.argtypes = [i32]; lib.pwpp_bind_host_to_device.restype = i32
@@ -966,6 +968,16 @@ class Engine:
         """ORDER_BIN (default): ascending point index inside a bin; ORDER_REFERENCE: the reference's z order, equal z in ascending
         point index; ORDER_REFERENCE_EXACT: the reference's z order with equal z as libstdc++'s std::sort leaves them (pwpp.h)."""
         _check(self.lib.pwpp_set_output_order(self._h, order))
+
+    ARITH_DOUBLE, ARITH_REFERENCE = 0, 1
+
+    def set_arithmetic(self, mode: int):
+        """ARITH_DOUBLE (default): order-free double sums; ARITH_REFERENCE: the reference's fp32 arithmetic, every result bit for
+        bit the reference build's (pwpp.h). Refused while a call is bound."""
+        _check(self.lib.pwpp_set_arithmetic(self._h, mode))
+
+    def arithmetic(self) -> int:
+        return self.lib.pwpp_arithmetic(self._h)
 
     def order_exact_counts(self, reset: bool = False):
         """Counters of the ORDER_REFERENCE_EXACT fix-up: (patches simulated, heap fall-backs, NaN bins); synchronises the device."""

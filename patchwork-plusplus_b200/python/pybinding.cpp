@@ -145,6 +145,13 @@ PYBIND11_MODULE(pypatchworkpp, m) {
       }, py::arg("order"),
            "\"bin\": ascending point index inside a bin; \"reference\" (default): the reference's order, equal z in ascending point "
            "index; \"reference_exact\": equal z where the reference's std::sort (libstdc++) leaves them")
+      .def("setArithmetic", [](patchwork::PatchWorkpp& s, const std::string& arith) {
+        if (arith == "double") s.setArithmetic(patchwork::Arithmetic::Double);
+        else if (arith == "reference") s.setArithmetic(patchwork::Arithmetic::Reference);
+        else throw py::value_error("arith must be \"double\" or \"reference\"");
+      }, py::arg("arith"),
+           "\"double\" (default): order-free double sums; \"reference\": the reference's fp32 arithmetic, every result bit for bit "
+           "the CPU library's")
       .def("getGroundIndicesDevice", [](py::object self) {
         auto& s = self.cast<patchwork::PatchWorkpp&>();
         const auto v = s.groundIndicesDevice();

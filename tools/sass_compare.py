@@ -20,9 +20,9 @@ for n, dn in zip(b, names):
     if n not in a: print("NEW      ", len(b[n]), short); continue
     same = a[n] == b[n]
     print("IDENTICAL" if same else "DIFFERENT", len(a[n]), len(b[n]), short)
-print("---- template kernels matched by dropping the new trailing 'false' parameter")
-da = {re.sub(r"\(.*", "", x).replace("void pwpp::", ""): a[n] for n, x in zip(a, subprocess.run(["c++filt"] + list(a), capture_output=True, text=True).stdout.split("\n"))}
-db = {re.sub(r"\(.*", "", x).replace("void pwpp::", ""): b[n] for n, x in zip(b, names)}
+print("---- template kernels matched by dropping the new trailing 'false' parameter (or the whole parameter list of a kernel that became a template)")
+da = {re.sub(r"\(.*", "", x).replace("void pwpp::", "").replace("pwpp::", ""): a[n] for n, x in zip(a, subprocess.run(["c++filt"] + list(a), capture_output=True, text=True).stdout.split("\n"))}
+db = {re.sub(r"\(.*", "", x).replace("void pwpp::", "").replace("pwpp::", ""): b[n] for n, x in zip(b, names)}
 for k, v in db.items():
     if k in da: continue
     k2 = k
