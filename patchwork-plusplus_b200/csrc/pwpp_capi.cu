@@ -1148,17 +1148,18 @@ static int create_impl(const pwpp_params* sets, int num_sets, const int32_t* str
     // Fit kernel of every patch-size class:
     //   S  <= 64      k_fit_resident: 8 lanes x 8 register slots per patch
     //   M  <= 512     k_fit_warp, patch staged in shared memory, plane + moment sums in shared memory, 3 CTAs/SM
-    //   L1 <= 2048    k_fit_warp streaming from L2, the same (4 CTAs/SM at 64 registers and a cp.async chunk ring were slower)
-    //                 Both are instruction-fetch sensitive (125 KB of code each): the passes take TWO rows per batch, the LPR scans two
-    //                 loads in flight (more rows per batch or more loads in flight were slower).
+    //                 Instruction-fetch sensitive (125 KB of code): the passes take TWO rows per batch, the LPR scans two loads in
+    //                 flight (more rows per batch or more loads in flight were slower).
+    //   L1 <= 2048    k_fit_warp, x, y, z staged in 24 KB of shared memory per warp: one CTA of 8 warps per SM, so the plane stays
+    //                 in registers and the R-VPF round is fused with the R-GPF seed fit (profiles/h100_fit_l1.jsonl)
     //                 PWPP_FIT_PATCH=1 (and calls of <= 4 frames): k_fit_patch, one patch per CTA of 4 / 8 / 16 warps held in registers
     //   L2 <= 4096    k_fit_cta, per-patch state in shared memory, 4 CTAs/SM
     //   L3 <= 8192    k_fit_cta, 2 CTAs/SM
     //   X  >  8192    k_fit_big (dense sensors)
-    const size_t sm_m = FITW_WARPS * CLS_M_MAX * sizeof(float4), sm_l2 = 3 * 4096 * sizeof(float), sm_l3 = 3 * 8192 * sizeof(float);
+    const size_t sm_m = FITW_SMEM_M, sm_l2 = 3 * 4096 * sizeof(float), sm_l3 = 3 * 8192 * sizeof(float);
     ctx->fit[0] = {k_fit_resident<8, 8, 0, 2>, 0, FIT_THREADS, 0};
     ctx->fit[1] = {k_fit_warp<true, 1, 1, 2, 3, false, true>, 0, FITW_WARPS * 32, sm_m};
-    ctx->fit[2] = {k_fit_warp<false, 2, 2, 2, 3, false, true>, 0, FITW_WARPS * 32, 0};
+    ctx->fit[2] = {k_fit_warp<true, 2, 2, 2, 1, true, false, true>, 0, FITW_WARPS * 32, FITW_SMEM_L1};
     ctx->fit[3] = {k_fit_cta<4096, 3, 4, 8, true, true>, 0, FIT_THREADS, sm_l2};
     ctx->fit[4] = {k_fit_cta<8192, 4, 2, 8, true>, 0, FIT_THREADS, sm_l3};
     ctx->fit[5] = {k_fit_big<16, 1, true>, 0, 512, 0};

@@ -7,8 +7,8 @@
 // work items (frame, bin, size, offset) from a device-side queue filled by k_bin_scan, so that every class keeps its points
 // in the fastest storage they fit in and re-reads HBM never:
 //     class S   n <= 64     k_fit_resident: 8 lanes x 8 points in registers, 4 patches per warp, no block barriers
-//     class M   n <= 512    k_fit_warp<STAGE>: one warp per patch, patch staged once in 8 KB of shared memory
-//     class L1  n <= 2048   k_fit_warp: one warp per patch, points streamed from L2, 4 loads in flight per lane
+//     class M   n <= 512    k_fit_warp<STAGE>: one warp per patch, float4 records staged once in 8 KB of shared memory
+//     class L1  n <= 2048   k_fit_warp<STAGE, SOA>: one warp per patch, x, y, z staged once in 24 KB of shared memory
 //     class L2  n <= 4096   k_fit_cta: one CTA per patch, SoA coordinates in 48 KB of shared memory
 //     class L3  n <= 8192   k_fit_cta: 96 KB of shared memory
 //     class X   n >  8192   k_fit_big (pwpp_fit_big.cuh): one CTA per patch streaming from L2 (dense sensors);
@@ -1024,11 +1024,15 @@ __device__ __forceinline__ bool is_alive(const RvpfPlanes& rv, double th_dist_v,
 }
 
 // ---------------------------------------------------------------------------------------------------
-// k_fit_warp: one warp per patch, no block-level synchronisation at all.
-//   STAGE = true  (class M, 65..512 points): the patch is copied once into the warp's 8 KB of shared memory and
-//                 every pass reads it from there;
-//   STAGE = false (classes L2 then L1, 513..8192 points): the points are streamed from L2 in every pass, four
-//                 independent 128-bit loads per lane in flight (lane l reads points l, l+32, ...).
+// k_fit_warp: one warp per patch, no block-level synchronisation at all. Lane l handles points l, l+32, ... of a pass.
+//   STAGE = true: the patch is copied once into the warp's own region of shared memory (FITW_U 128-bit loads per lane in
+//                 flight) and every pass reads it from there. A class's work items never hold more than its CAP points,
+//                 which bounds every shared-memory index by the patch's own n.
+//     SOA = false (class M, 65..512 points): the float4 records, 8 KB per warp;
+//     SOA = true  (class L1, 513..2048 points): x, y and z as three fp32 planes, 24 KB per warp. The index word is read
+//                 from global memory once, by the output pass.
+//   STAGE = false (classes L2 then L1): the points are streamed from L2 in every pass. The library no longer launches
+//                 this form; the SIMT twin's launch sequence (tests/simt/simt_twin.cpp) still runs class L1 on it.
 // Per point a pass must remember one bit, kept as the ballot word of its iteration in per-warp shared memory
 // (alive = not removed by R-VPF, S:495-504; member = in the set the current plane was fitted to).
 //
@@ -1042,10 +1046,16 @@ __device__ __forceinline__ bool is_alive(const RvpfPlanes& rv, double th_dist_v,
 constexpr int WARP_CAP = CLS_L3_MAX;            // 8192 points -> 256 iterations
 constexpr int FITW_WARPS = 8;
 constexpr int FITW_U = 4;                       // loads in flight per lane
+// dynamic shared memory of a k_fit_warp CTA: class M / class L1
+constexpr size_t FITW_SMEM_M = (size_t) FITW_WARPS * CLS_M_MAX * sizeof(float4);
+constexpr size_t FITW_SMEM_L1 = (size_t) FITW_WARPS * 3 * CLS_L1_MAX * sizeof(float);
 
 // Rare path of warp_lpr (num_lpr > 32, or more than 128 points tie below the bound): streaming selector with a
 // bitonic sort of the candidate buffer. Kept out of line so that its ~2000 instructions stay out of the hot code.
-__device__ __noinline__ double warp_lpr_fallback(const float4* __restrict__ P, int n, int nit, bool any_removed, const unsigned* __restrict__ alive_w,
+__device__ __forceinline__ float z_of(const float4& p) { return p.z; }
+__device__ __forceinline__ float z_of(float z) { return z; }
+template <typename PT>
+__device__ __noinline__ double warp_lpr_fallback(const PT* __restrict__ P, int n, int nit, bool any_removed, const unsigned* __restrict__ alive_w,
                                                  float margin_f, int num_lpr, float* sel_buf) {
   const int lane = lane_id();
   double lpr = 0.0;
@@ -1054,7 +1064,7 @@ __device__ __noinline__ double warp_lpr_fallback(const float4* __restrict__ P, i
   for (int it = 0; it < nit; ++it) {
     const int j = it * 32 + lane;
     bool valid = j < n;
-    const float z = P[j < n ? j : n - 1].z;
+    const float z = z_of(P[j < n ? j : n - 1]);
     if (any_removed) valid = valid && ((alive_w[it] >> lane) & 1u);
     if (z < margin_f) valid = false;
     sel.push(valid, z);
@@ -1074,8 +1084,9 @@ __device__ __noinline__ double warp_lpr_fallback(const float4* __restrict__ P, i
 // Two-level selection: the num_lpr-th smallest of the 32 per-lane minima is an upper bound T of the num_lpr-th
 // smallest point, so only the few points with z <= T are gathered (ballot append into the warp's 128-slot buffer)
 // and the exact k-th key is bisected among them. Falls back to the streaming selector when num_lpr > 32 or when
-// more than 128 points tie below the bound.
-__device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool any_removed, const unsigned* __restrict__ alive_w, float margin_f,
+// more than 128 points tie below the bound. P: the patch's float4 records or its z plane.
+template <typename PT>
+__device__ double warp_lpr(const PT* __restrict__ P, int n, int nit, bool any_removed, const unsigned* __restrict__ alive_w, float margin_f,
                            int num_lpr, float* sel_buf) {
   const int lane = lane_id();
   const unsigned lt = lanemask_lt();
@@ -1092,7 +1103,7 @@ __device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool an
     for (int it0 = 0; it0 < nit; it0 += LPR_U) {
       float zb[LPR_U];
 #pragma unroll
-      for (int u = 0; u < LPR_U; ++u) { const int j = (it0 + u) * 32 + lane; zb[u] = P[j < n ? j : n - 1].z; }
+      for (int u = 0; u < LPR_U; ++u) { const int j = (it0 + u) * 32 + lane; zb[u] = z_of(P[j < n ? j : n - 1]); }
 #pragma unroll
       for (int u = 0; u < LPR_U; ++u) {
         const int it = it0 + u, j = it * 32 + lane;
@@ -1117,7 +1128,7 @@ __device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool an
     for (int it0 = 0; it0 < nit; it0 += LPR_U) {
       float zb[LPR_U];
 #pragma unroll
-      for (int u = 0; u < LPR_U; ++u) { const int j = (it0 + u) * 32 + lane; zb[u] = P[j < n ? j : n - 1].z; }
+      for (int u = 0; u < LPR_U; ++u) { const int j = (it0 + u) * 32 + lane; zb[u] = z_of(P[j < n ? j : n - 1]); }
 #pragma unroll
       for (int u = 0; u < LPR_U; ++u) {
         const int it = it0 + u, j = it * 32 + lane;
@@ -1167,18 +1178,20 @@ __device__ double warp_lpr(const float4* __restrict__ P, int n, int nit, bool an
 // PLS: the current plane and the running moment sums of a warp's patch live in shared memory (160 B per warp) instead of ~40
 // registers per lane: the passes only need the plane as four floats (PlaneF), the doubles are read in the rare exact distance
 // test and by the solve. That is what lets the kernel run at 3 CTAs per SM (85 registers) without spilling.
-template <bool STAGE, int CLS_HI, int CLS_LO, int U, int MINB, bool FUSE = false, bool PLS = false>
+template <bool STAGE, int CLS_HI, int CLS_LO, int U, int MINB, bool FUSE = false, bool PLS = false, bool SOA = false>
 __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4* __restrict__ sorted, FrameTable ft, const StreamState* __restrict__ states,
                                                                              const __grid_constant__ GeometrySets gs, const __grid_constant__ AlgoParamSets aps, int nbp, const int* __restrict__ bin_off, WorkQueues wq,
                                                                              int* __restrict__ part, BinFit* __restrict__ fits) {
-  constexpr int CAP = STAGE ? CLS_M_MAX : (CLS_HI == 2 ? CLS_L1_MAX : WARP_CAP);
+  constexpr int CAP = STAGE ? (SOA ? CLS_L1_MAX : CLS_M_MAX) : (CLS_HI == 2 ? CLS_L1_MAX : WARP_CAP);
+  static_assert(!SOA || STAGE, "the x, y, z planes are a staging layout");
+  static_assert(!STAGE || (CLS_HI == (SOA ? 2 : 1) && CLS_LO <= CLS_HI), "the largest class drained must fit the staging region");
   __shared__ unsigned s_alive[FITW_WARPS][CAP / 32];
   __shared__ unsigned s_member[FITW_WARPS][CAP / 32];
   __shared__ float s_sel[FITW_WARPS][128];
   __shared__ Plane s_pl[PLS ? FITW_WARPS : 1];
   __shared__ Moments s_tot[PLS ? FITW_WARPS : 1];
   static_assert(!(PLS && FUSE), "the fused seed round keeps two planes in registers");
-  PW_DYN_SHARED(float4, s_stage);              // STAGE: [FITW_WARPS][CLS_M_MAX]
+  PW_DYN_SHARED(float4, s_stage);              // STAGE: [FITW_WARPS][CAP] records, or with SOA [FITW_WARPS][3][CAP] floats
   const int warp = threadIdx.x >> 5, lane = lane_id();
   const unsigned lt = lanemask_lt();
   unsigned* alive_w = s_alive[warp];
@@ -1220,8 +1233,11 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
     const float4* G = sorted + start;           // the patch in global memory
     int* out = part + start;
     const int nit = (n + 31) >> 5;
-    const float4* P = G;                        // where the passes read the points from
-    if (STAGE) {
+    const float4* P = G;                        // where the passes read the points from (unless SOA)
+    float* const px = reinterpret_cast<float*>(s_stage) + warp * 3 * CAP;   // SOA: the warp's x, y, z planes
+    float* const py = px + CAP;
+    float* const pz = py + CAP;
+    if (STAGE && !SOA) {
       float4* mine = s_stage + warp * CLS_M_MAX;
       for (int it = 0; it < nit; it += FITW_U) {   // global loads: always FITW_U in flight
         float4 q[FITW_U];
@@ -1232,12 +1248,23 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
       }
       __syncwarp();
       P = mine;
+    } else if (SOA) {
+      for (int it = 0; it < nit; it += FITW_U) {
+        float4 q[FITW_U];
+#pragma unroll
+        for (int u = 0; u < FITW_U; ++u) { const int j = (it + u) * 32 + lane; q[u] = G[j < n ? j : n - 1]; }
+#pragma unroll
+        for (int u = 0; u < FITW_U; ++u) { const int j = (it + u) * 32 + lane; if (j < n) { px[j] = q[u].x; py[j] = q[u].y; pz[j] = q[u].z; } }
+      }
+      __syncwarp();
     }
+    // point j (j < n) as the passes see it; .w only holds the index outside the SOA layout
+    auto pt = [&](int j) -> float4 { if constexpr (!SOA) return P[j]; else return make_float4(px[j], py[j], pz[j], 0.f); };
     const int zone = (bin >= g.bin_base[3]) ? 3 : (bin >= g.bin_base[2]) ? 2 : (bin >= g.bin_base[1]) ? 1 : 0;
     const bool zone0 = (zone == 0);
     // S:90; (double) z < margin  <=>  z < margin_f (float_ru), folded with the zone-0 condition
     const float margin_f = zone0 ? float_ru(ap.adaptive_seed_selection_margin * states[ft.stream[f]].sensor_height) : -INFINITY;
-    const float4 first = P[0];
+    const float4 first = pt(0);
     double c[3] = {(double) first.x, (double) first.y, 0.0};   // reference point of all moment sums of this patch
 
     bool have_plane = false, any_removed = false;
@@ -1270,7 +1297,9 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
       const bool rvpf_round = rvpf_left > 0;
       const bool fused = fuse_ok && rvpf_round;
       // LPR: mean of the num_lpr lowest z among the alive points not below the zone-0 margin (S:88-103)
-      const double lpr = warp_lpr(P, n, nit, any_removed, alive_w, margin_f, ap.num_lpr, sel_buf);
+      double lpr;
+      if constexpr (!SOA) lpr = warp_lpr(P, n, nit, any_removed, alive_w, margin_f, ap.num_lpr, sel_buf);
+      else lpr = warp_lpr(pz, n, nit, any_removed, alive_w, margin_f, ap.num_lpr, sel_buf);
       const float zthr = float_ru(lpr + (rvpf_round ? ap.th_seeds_v : ap.th_seeds));
       const float zin = float_ru(lpr + ap.th_seeds);   // inner (R-GPF seed) threshold of a fused round
       c[2] = lpr;
@@ -1289,7 +1318,7 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
       for (int it = 0; it < nit; it += U) {
         float4 q[U];
 #pragma unroll
-        for (int u = 0; u < U; ++u) { const int j = (it + u) * 32 + lane; q[u] = P[j < n ? j : n - 1]; }
+        for (int u = 0; u < U; ++u) { const int j = (it + u) * 32 + lane; q[u] = pt(j < n ? j : n - 1); }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int j = (it + u) * 32 + lane;
@@ -1356,7 +1385,7 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
         for (int it = 0; it < nit; ++it) {
           const int j = it * 32 + lane;
           bool keep = j < n;
-          const float4 p = P[j < n ? j : n - 1];
+          const float4 p = pt(j < n ? j : n - 1);
           if (any_removed) keep = keep && ((alive_w[it] >> lane) & 1u);
           const bool was_alive = keep;
           keep = keep && !(fabs(point_plane_distance(pl, p.x, p.y, p.z)) < ap.th_dist_v);   // S:499
@@ -1386,7 +1415,7 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
       for (int it = 0; it < nit; it += U) {
         float4 q[U];
 #pragma unroll
-        for (int u = 0; u < U; ++u) { const int j = (it + u) * 32 + lane; q[u] = P[j < n ? j : n - 1]; }
+        for (int u = 0; u < U; ++u) { const int j = (it + u) * 32 + lane; q[u] = pt(j < n ? j : n - 1); }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           if (it + u >= nit) break;
@@ -1432,11 +1461,12 @@ __global__ void __launch_bounds__(FITW_WARPS * 32, MINB) k_fit_warp(const float4
     __syncwarp();
     // stable partition: ground indices ascending, then non-ground indices ascending
     {
+      const float4* I = SOA ? G : P;            // the records that hold the point indices
       int g_run = 0, ng_run = 0;
       for (int it0 = 0; it0 < nit; it0 += U) {   // U index loads in flight per lane
         int idxb[U];
 #pragma unroll
-        for (int u = 0; u < U; ++u) { const int j = (it0 + u) * 32 + lane; idxb[u] = __float_as_int(P[j < n ? j : n - 1].w); }
+        for (int u = 0; u < U; ++u) { const int j = (it0 + u) * 32 + lane; idxb[u] = __float_as_int(I[j < n ? j : n - 1].w); }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int it = it0 + u, j = it * 32 + lane;

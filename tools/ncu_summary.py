@@ -20,7 +20,7 @@ COLS = ["Kernel Name", "Block Size", "Grid Size", "gpu__time_duration.sum", "dra
 
 # kernel name -> the stage name bench.py uses
 STAGES = [(r"k_front_cluster", "k_front"), (r"k_bin_hist", "k_bin_hist"), (r"k_bin_scan", "k_bin_scan"), (r"k_scatter", "k_scatter"),
-          (r"k_fit_resident", "k_fit_S"), (r"k_fit_warp<\(bool\)1|k_fit_warp<1", "k_fit_M"), (r"k_fit_warp<\(bool\)0|k_fit_warp<0", "k_fit_L1"),
+          (r"k_fit_resident", "k_fit_S"), (r"k_fit_warp<\(bool\)1, \(int\)1|k_fit_warp<1, 1", "k_fit_M"), (r"k_fit_warp<", "k_fit_L1"),
           (r"k_fit_cta<4096|k_fit_cta<\(int\)4096", "k_fit_L2"), (r"k_fit_cta<8192|k_fit_cta<\(int\)8192", "k_fit_L3"),
           (r"k_fit_patch<4|k_fit_patch<\(int\)4", "k_fit_L1"), (r"k_fit_patch<8|k_fit_patch<\(int\)8", "k_fit_L2"),
           (r"k_fit_patch<16|k_fit_patch<\(int\)16", "k_fit_L3"), (r"k_fit_big", "k_fit_X"), (r"k_gle", "k_gle"), (r"k_order", "k_order"),
